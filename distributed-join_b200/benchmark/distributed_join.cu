@@ -1,5 +1,5 @@
 // distributed_join.cu -- the reference's synthetic join benchmark (benchmark/distributed_join.cu)
-// built against the B200 library.  Same flags, same parameter report, same "Elasped time (s)"
+// built against libdj_b200.  Same flags, same parameter report, same "Elasped time (s)"
 // line; MPI calls are replaced by dj_bootstrap (ranks come from RANK/WORLD_SIZE), row counts are
 // 64-bit, and a JSON line with rows/s is printed next to the reference's output.
 //

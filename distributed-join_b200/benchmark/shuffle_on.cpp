@@ -48,10 +48,12 @@ int main(int argc, char* argv[])
   setup_memory_pool_and_communicator(communicator, registered_mr, pool_mr, "NCCL", "none", 0);
   const int rank = communicator->mpi_rank, size = communicator->mpi_size;
 
-  // four int64 columns: random keys (the generator's duplicate-allowed build stream) + 3 payloads
+  // four int64 columns: random keys (the generator's duplicate-allowed build stream) + 3 payloads.
+  // Keys come from [0, 2^34]: that stream keeps a bitmap of rand_max + 1 bits (2 GB here), which has
+  // to fit on an 80 GB GPU next to the table and its shuffled copy.
   std::unique_ptr<cudf::table> kp, unused;
   std::tie(kp, unused) = generate_build_probe_tables<int64_t, int64_t>((cudf::size_type)rows_per_rank, 1, 0.0,
-                                                                       (int64_t)1 << 40, false, rank);
+                                                                       (int64_t)1 << 34, false, rank);
   std::vector<std::unique_ptr<cudf::column>> cols;
   {
     auto v = kp->view();

@@ -1,4 +1,4 @@
-// dj_device.cuh -- device-side primitives shared by the sm_100a kernels:
+// dj_device.cuh -- device-side primitives shared by the sm_90a kernels:
 // hashes, Philox / Feistel generator pieces, block scan, launch bookkeeping.
 #pragma once
 
@@ -89,7 +89,7 @@ __host__ __device__ __forceinline__ uint32_t row_hash_i64(int64_t key, uint32_t 
 // Hash used for the join's private radix sub-partitioning; the radix levels consume its TOP bits.
 // It must be independent of the rank-partition hash (rows on one rank share row_hash % nparts) but
 // is otherwise free: two 64-bit multiplies with an xor-shift between them (about half the
-// instructions of murmur3 -- the scatter kernels are issue-bound, profiles/r02a_summary.md).
+// instructions of murmur3: the scatter kernels spend their time issuing instructions, not waiting on HBM).
 __host__ __device__ __forceinline__ uint32_t local_hash_i64(int64_t key)
 {
   uint64_t x = (uint64_t)key * 0x9E3779B97F4A7C15ull;

@@ -1,4 +1,4 @@
-// join.cu -- shared-memory open-addressing hash build + probe for sm_100a.
+// join.cu -- shared-memory open-addressing hash build + probe for sm_90a (H100).
 //
 // Replaces cudf::inner_join as called by local_join_helper (src/distributed_join.cpp:71-83).
 // Both tables arrive radix-partitioned (partition.cu, mode 1) into buckets whose build side
@@ -20,9 +20,6 @@
 //                      stores; the atomic's round trip is hidden behind the next round of probing
 //                      (three tiles rotate), and batch results land in one output so no
 //                      cudf::concatenate is needed afterwards.
-// Tried and rejected (measured on B200, 800M x 800M): replacing the two consumer bar.sync phases by
-// split arrive/wait mbarriers so that early warps start the next table's inserts -- 16.0 -> 20.0 ms
-// (inserts then contend with probes for the atomic unit and the mbarrier polls cost issue slots).
 // Multimap semantics: probing continues past a hit until an empty slot.  Build buckets larger
 // than one chunk (skew / duplicates) are processed chunk by chunk, re-streaming the probe side.
 #include <cstdlib>

@@ -1,4 +1,4 @@
-// partition.cu -- radix / hash partition passes for sm_100a.
+// partition.cu -- radix / hash partition passes for sm_90a (H100).
 //
 // One "pass" splits every parent bucket (a contiguous row range of SoA int64 columns) into
 // F child buckets, in three stream-ordered launches and no host synchronisation:
@@ -525,7 +525,7 @@ __global__ void __launch_bounds__(THREADS, 1) scatter_tma_kernel(PassDev d)
 // out.  One persistent 1024-thread CTA per SM; per 4096-row tile:
 //   TMA      the tile arrives in shared memory two tiles ahead (cp.async.bulk + mbarrier);
 //   rank     every row: bucket = hash bits, rank = shared-memory atomicAdd on the bucket's counter
-//            (measured 3.9 cycles per 32 rows at 512-1024 buckets, experiments/mb_smem_rank.cu);
+//            (experiments/mb_smem_rank.cu compares it with warp-aggregated ranking);
 //   reserve  one thread per bucket: global atomicAdd reserves the run's slice of the bucket (the
 //            result is not needed until the copy-out), block scan of the counters;
 //   sort     every row is written to its bucket-sorted position as one STS.128;

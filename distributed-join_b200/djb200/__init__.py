@@ -2,7 +2,7 @@
 
 PyTorch is used only as plumbing: device memory (tensors), streams and torch.distributed for
 process launch / unique-id broadcast.  Every compute call goes through the C ABI into the
-hand-written sm_100a kernels; there is NO CPU or PyTorch fallback -- if the shared library is
+hand-written sm_90a kernels; there is NO CPU or PyTorch fallback -- if the shared library is
 missing or a call fails this module raises.
 """
 from __future__ import annotations

@@ -59,10 +59,10 @@ void append_to_all_to_all_comm_buffers(cudf::table_view input, cudf::mutable_tab
   for (cudf::size_type c = 0; c < input.num_columns(); c++) {
     const cudf::data_type dtype = input.column(c).type();
     if (!cudf::is_fixed_width(dtype))
-      throw std::runtime_error("all-to-all: only fixed-width columns are supported by the B200 build");
+      throw std::runtime_error("all-to-all: only fixed-width columns are supported by this build");
     if ((size_t)c < compression_options.size() &&
         compression_options[c].compression_method != CompressionMethod::none)
-      throw std::runtime_error("all-to-all: compression is not supported by the B200 build");
+      throw std::runtime_error("all-to-all: compression is not supported by this build");
     buffers.emplace_back(input.column(c).head(), output.column(c).head(), send64, recv_offsets, dtype);
   }
 }

@@ -1,7 +1,7 @@
 // compression.hpp -- signature-compatible placeholder for the reference's nvcomp options
 // (src/compression.hpp:45-58, src/compression.cpp:75-95).  Compression is out of scope: nvcomp
-// is not in the image, the benchmark default is off (benchmark/distributed_join.cu:107) and at
-// 900 GB/s per direction it costs more than it saves.  Only `none` exists.
+// is not a dependency, the benchmark default is off (benchmark/distributed_join.cu:107) and at
+// H100 NVLink rates (450 GB/s per direction) it costs more than it saves.  Only `none` exists.
 #pragma once
 
 #include <stdexcept>
@@ -24,7 +24,7 @@ inline std::vector<ColumnCompressionOptions> generate_compression_options_distri
   cudf::table_view input_table, bool compression)
 {
   if (compression)
-    throw std::runtime_error("compression is not supported by the B200 build (NVLink 5 makes it a loss)");
+    throw std::runtime_error("compression is not supported by this build (over NVLink it costs more than it saves)");
   return generate_none_compression_options(input_table);
 }
 

@@ -10,7 +10,7 @@ void require_fixed_width(table_view const& t, const char* what)
 {
   for (auto const& c : t)
     if (!is_fixed_width(c.type()))
-      throw std::runtime_error(std::string(what) + ": the B200 build handles fixed-width columns only");
+      throw std::runtime_error(std::string(what) + ": this build handles fixed-width columns only");
 }
 
 __global__ void widen_kernel(const int32_t* in, int64_t* out, int64_t n)
@@ -23,7 +23,7 @@ __global__ void narrow_kernel(const int64_t* in, int32_t* out, int64_t n)
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     out[i] = (int32_t)in[i];
 }
-int grid_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 148 * 16)); }
+int grid_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 132 * 16)); }
 }  // namespace
 
 bool all_i64(table_view const& t)

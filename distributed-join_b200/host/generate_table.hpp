@@ -32,7 +32,7 @@ std::pair<std::unique_ptr<cudf::table>, std::unique_ptr<cudf::table>> generate_b
   int64_t nb_total = -1, int64_t np_total = -1)
 {
   static_assert(std::is_same<KEY_T, int64_t>::value && std::is_same<PAYLOAD_T, int64_t>::value,
-                "the B200 build generates int64 keys and payloads");
+                "this build generates int64 keys and payloads");
   dj_gen_params g{};
   g.nb                = nb_total < 0 ? build_table_nrows : nb_total;
   g.np                = np_total < 0 ? probe_table_nrows : np_total;

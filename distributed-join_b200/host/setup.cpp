@@ -26,7 +26,7 @@ void setup_memory_pool_and_communicator(
 {
   registered_mr = nullptr;
   if (communicator_name != "NCCL")
-    throw std::runtime_error("Unknown communicator name (the B200 build provides \"NCCL\" only; UCX is out of scope)");
+    throw std::runtime_error("Unknown communicator name (this build provides \"NCCL\" only; UCX is out of scope)");
   size_t free_memory = 0, total_memory = 0;
   CUDA_RT_CALL(cudaMemGetInfo(&free_memory, &total_memory));
   const size_t pool_size = free_memory / 284 * 256;  // same sizing rule as src/setup.cpp:64

@@ -1,5 +1,5 @@
 // compare_against_analytical.cu -- the reference's analytical integration test
-// (test/compare_against_analytical.cu) against the B200 library: left keys 0,3,6,..., right keys
+// (test/compare_against_analytical.cu) against libdj_b200: left keys 0,3,6,..., right keys
 // 0,5,10,..., payload = row id; after distributed_inner_join the global row count must be
 // size/5 and every row must satisfy  key%15==0, left payload == key/3, right payload == key/5.
 // Each rank holds a contiguous slice (what distribute_table would hand it).

@@ -1,5 +1,5 @@
 // compare_against_single_gpu.cu -- the reference's strongest integration test
-// (test/compare_against_single_gpu.cu:96-205,237-268) against the B200 library: rank 0 generates
+// (test/compare_against_single_gpu.cu:96-205,237-268) against libdj_b200: rank 0 generates
 // build / probe tables with the known-selectivity generator and joins them on ONE GPU; the tables
 // are dealt to all ranks with distribute_table, joined with distributed_inner_join, gathered with
 // collect_tables, and both results must be the same row multiset (sorted, compared element-wise).
@@ -126,7 +126,7 @@ int main(int argc, char* argv[])
   ok &= run_test(I64, type_id::DURATION_MICROSECONDS, 1'000'000, 1'000'000, 0.3, true, 1, 1, communicator);
   ok &= run_test(I32, I32, 1'000'000, 1'000'000, 0.3, true, 1, 2, communicator);
   ok &= run_test(I32, I32, 1'000'000, 1'000'000, 0.3, true, 10, 2, communicator);
-  // beyond the reference's list: the whole NVLink domain (the fused B200 path) and duplicate build keys
+  // beyond the reference's list: the whole NVLink domain (the fused path) and duplicate build keys
   ok &= run_test(I64, I64, 1'000'000, 5'000'000, 0.3, true, 10, communicator->mpi_size, communicator);
   ok &= run_test(I64, I64, 1'000'000, 5'000'000, 0.9, false, 4, communicator->mpi_size, communicator);
   ok &= run_test(I32, I64, 2'000'000, 2'000'000, 0.3, true, 1, communicator->mpi_size, communicator);

@@ -1,5 +1,5 @@
 /*
- * dj_b200.h -- C ABI of libdj_b200.so, the B200-native (sm_100a) replacement for the device
+ * dj_b200.h -- C ABI of libdj_b200.so, the H100-native (sm_90a) replacement for the device
  * side of rapidsai/distributed-join's hot path:
  *
  *     hash-partition  ->  all-to-all  ->  local hash join

@@ -32,7 +32,7 @@
  * bit-equal against sklearn.utils.murmurhash3_32 (tests/golden/murmur3_kat.json).
  * PARITY UNPINNED for the key -> partition-id assignment only: no reference test pins it
  * (test/test_shuffle_on.cpp:78-83 uses HASH_IDENTITY and checks congruence only) and cuDF
- * 0.19's row_hasher is not in /root/reference.  Join results are invariant to it.
+ * 0.19's row_hasher is not in the reference tree.  Join results are invariant to it.
  */
 #include <stdint.h>
 #include <stdlib.h>

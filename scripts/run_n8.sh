@@ -1,11 +1,12 @@
 #!/bin/bash
-# One-box multi-GPU validation + numbers: NP=8 scripts/run_n8.sh   (writes gpurun_out/r02_n${NP}_*.log)
+# One-node multi-GPU validation + numbers: NP=8 scripts/run_n8.sh   (writes ${OUT:-run_n8_out}/n${NP}_*.log)
 cd "$(dirname "$0")/.."
 NP=${NP:-8}
-mkdir -p gpurun_out
+OUTDIR=${OUT:-run_n8_out}
+mkdir -p $OUTDIR
 TRP="python -m torch.distributed.run --nnodes=1 --nproc-per-node $NP --master-addr 127.0.0.1"
 F='^\*\|OMP_NUM\|^$\|W09'
-O=gpurun_out/r02_n${NP}
+O=$OUTDIR/n${NP}
 echo "== parity (python, oracle-checked)"; timeout 400 $TRP --master-port 29701 tests/test_multi_gpu.py 2>&1 | grep -v "$F" | tee ${O}_multigpu_parity.log | tail -16
 echo "== timeline"; timeout 200 $TRP --master-port 29709 scripts/trace_timeline.py 2>&1 | grep "trace rank [07]" | tee ${O}_trace.log | grep "rank 0"
 echo "== bench"; timeout 500 $TRP --master-port 29702 bench.py --gpus $NP --steps 5 --warmup 3 2>&1 | grep -v "$F" | tail -2 | tee ${O}_bench.json | cut -c1-3500

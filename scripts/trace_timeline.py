@@ -7,7 +7,7 @@ rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
 torch.cuda.set_device(rank); dev = torch.device("cuda", rank)
 dist.init_process_group("nccl", device_id=dev)
 comm = dj.Comm.from_torch_distributed()
-n = int(os.environ.get("DJ_TRACE_ROWS", 800_000_000)) // world
+n = int(os.environ.get("DJ_TRACE_ROWS", 400_000_000)) // world
 g = dj.gen_params(n, n, 0.3, 2 * n, True)
 (lk, lp), (rk, rp) = dj.generate_tables_distributed(g, rank, world, dev)
 cap = int(n * 0.35) + 1_000_000

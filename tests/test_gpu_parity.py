@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a kernels, called through the C ABI (libdj_b200.so via ctypes),
+"""GPU parity tests: the sm_90a kernels, called through the C ABI (libdj_b200.so via ctypes),
 against the CPU oracle on the same seeded inputs.  Integer work -> bit-exact."""
 import json
 import os
