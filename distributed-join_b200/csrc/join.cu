@@ -204,8 +204,16 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
               k = (int64_t)(((uint64_t)(uint32_t)pr.y << 32) | (uint32_t)pr.x);
               v = (int64_t)(((uint64_t)(uint32_t)pr.w << 32) | (uint32_t)pr.z);
             }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s.empty_probe[st]);  // rows are in registers: release
+            // Release the stage only once every lane's row has LANDED in registers: neither __syncwarp
+            // nor the arrive waits for an outstanding shared-memory load, and the producer's next TMA
+            // copy into this stage (async proxy) is not ordered after it, so it could overwrite a row
+            // a lane had not read yet (that lane then probed a row of the chunk two ahead twice).  The
+            // reduction consumes the loaded registers, and the arrive depends on its (always nonzero)
+            // result.
+            const unsigned landed =
+              __reduce_and_sync(0xffffffffu, (uint32_t)((uint64_t)k ^ ((uint64_t)k >> 32) ^ (uint64_t)v ^
+                                                        ((uint64_t)v >> 32)) | 1u);
+            if (lane == 0 && landed) mbar_arrive(&s.empty_probe[st]);
             q++;
 
             const uint32_t h    = slot_hash_i64(k);

@@ -196,16 +196,23 @@ def hash_partition(keys, payloads, nparts, seed=SEED_NVLINK, hash_id=HASH_MURMUR
     return ko, pos, offsets
 
 
-def inner_join(bk, bp, pk, pp, capacity=None, ws=None):
+def inner_join(bk, bp, pk, pp, capacity=None, ws=None, outs=None):
     """cudf::inner_join replacement on device tensors.
-    Returns ((build key, build payload, probe key, probe payload) trimmed to n_out, n_out)."""
+    Returns ((build key, build payload, probe key, probe payload) trimmed to n_out, n_out).
+    `outs`: four caller-owned columns for the first attempt (at least `capacity` rows each); when
+    the result does not fit, they keep the truncated first attempt and the retry gets new ones."""
     bk, bp, pk, pp = map(_i64dev, (bk, bp, pk, pp))
     nb, np_ = bk.numel(), pk.numel()
     if capacity is None:
         capacity = max(np_, 1)
     dev = bk.device
+    if outs is not None:
+        outs = list(map(_i64dev, outs))
+        if min(o.numel() for o in outs) < capacity:
+            raise DjError("inner_join: output columns are shorter than the capacity")
     while True:
-        outs = [torch.empty(capacity, dtype=torch.int64, device=dev) for _ in range(4)]
+        if outs is None:
+            outs = [torch.empty(capacity, dtype=torch.int64, device=dev) for _ in range(4)]
         cnt = torch.zeros(1, dtype=torch.int64, device=dev)
         if ws is None:
             ws = workspace(lib().dj_inner_join_workspace_bytes(nb, np_), dev)
@@ -215,6 +222,7 @@ def inner_join(bk, bp, pk, pp, capacity=None, ws=None):
         if n <= capacity:
             return tuple(o[:n] for o in outs), n
         capacity = n  # exact retry, as dj_b200.h documents
+        outs = None
 
 
 def gen_params(nb, np_, selectivity, rand_max, unique=True, seed=GEN_SEED) -> GenParams:

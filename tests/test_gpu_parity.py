@@ -34,19 +34,32 @@ def test_partition_ids_match_oracle_and_golden(dj, oracle):
         assert (got == oracle.partition_ids(keys, 12345678, nparts, hid)).all()
 
 
-@pytest.mark.parametrize("n,nparts,npay", [(0, 8, 1), (1, 8, 1), (4095, 8, 1), (4097, 2, 1), (250_000, 8, 1),
-                                           (250_000, 32, 1), (100_003, 7, 2), (100_003, 64, 3),
-                                           (1_000_000, 1024, 1), (3_000_000, 8, 1)])
-def test_hash_partition_matches_oracle(dj, oracle, n, nparts, npay):
+MURMUR3, IDENTITY = 1, 0  # DJ_HASH_MURMUR3 / DJ_HASH_IDENTITY
+_HP_CASES = [(0, 8, 1), (1, 8, 1), (4095, 8, 1), (4097, 2, 1), (250_000, 8, 1), (250_000, 32, 1), (100_003, 7, 2),
+             (100_003, 64, 3), (1_000_000, 1024, 1), (3_000_000, 8, 1)]
+# edges: a single partition; non-power-of-two fan-outs with one payload column (the TMA kernel's `%`
+# path, warp-aggregated for F <= 32 and per-row above); the identity hash on negative keys; one row
+# either side of the 32768-row histogram tile
+_HP_EDGES = [(10_000, 1, 1, MURMUR3), (50_000, 5, 1, MURMUR3), (50_000, 100, 1, MURMUR3), (50_000, 1000, 1, MURMUR3),
+             (200_000, 1024, 1, IDENTITY), (32_767, 8, 1, MURMUR3), (32_769, 100, 2, MURMUR3)]
+
+
+@pytest.mark.parametrize("n,nparts,npay,hid",
+                         [pytest.param(*c, MURMUR3, id="-".join(map(str, c))) for c in _HP_CASES] +
+                         [pytest.param(*c, id="-".join(map(str, c[:3])) + ("-identity" if c[3] == IDENTITY else ""))
+                          for c in _HP_EDGES])
+def test_hash_partition_matches_oracle(dj, oracle, n, nparts, npay, hid):
     """cudf::hash_partition contract: offsets bit-identical, each partition equal as a multiset."""
     rng = np.random.default_rng(n + nparts)
     keys = rng.integers(-(1 << 62), 1 << 62, n, dtype=np.int64)
+    if hid == IDENTITY:
+        keys = -np.abs(keys) - 1
     pays = [np.arange(n, dtype=np.int64) * (c + 1) + c for c in range(npay)]
-    ko, pos, off = dj.hash_partition(_t(keys), [_t(p) for p in pays], nparts, dj.SEED_NVLINK)
+    ko, pos, off = dj.hash_partition(_t(keys), [_t(p) for p in pays], nparts, dj.SEED_NVLINK, hid)
     ko, pos, off = _n(ko), [_n(p) for p in pos], _n(off)
-    ok, op, ooff = oracle.hash_partition(keys, pays[0], nparts, oracle.SEED_NVLINK)
+    ok, op, ooff = oracle.hash_partition(keys, pays[0], nparts, oracle.SEED_NVLINK, hid)
     assert (off == ooff).all()
-    ids = oracle.partition_ids(ko, oracle.SEED_NVLINK, nparts) if n else np.empty(0, np.int32)
+    ids = oracle.partition_ids(ko, oracle.SEED_NVLINK, nparts, hid) if n else np.empty(0, np.int32)
     for p in range(nparts):
         assert (ids[off[p]:off[p + 1]] == p).all()
         a = np.sort(pos[0][off[p]:off[p + 1]])
@@ -175,8 +188,11 @@ def test_full_size_properties_100m(dj, oracle):
     assert n2 == hits and dj.multiset_checksum4(cols2[2], cols2[3], cols2[0], cols2[1]) == ck
 
 
-def test_multi_gpu_parity_under_torchrun():
-    """N >= 2 ranks over NCCL (skipped on a single-GPU box): tests/test_multi_gpu.py under torchrun."""
+@pytest.mark.parametrize("env", [{}, {"DJ_EXCHANGE": "fused"}, {"DJ_NO_FUSE": "1"}],
+                         ids=["default", "exchange-fused", "no-fuse"])
+def test_multi_gpu_parity_under_torchrun(env):
+    """N >= 2 ranks over NCCL (skipped on a single-GPU box): tests/test_multi_gpu.py under torchrun, with
+    the default exchange, the fused partition + exchange kernel, and the unfused first radix level."""
     import socket
     import subprocess
     import sys
@@ -194,6 +210,6 @@ def test_multi_gpu_parity_under_torchrun():
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={n}",
                         "--master-addr", "127.0.0.1", "--master-port", str(port),
                         os.path.join("tests", "test_multi_gpu.py")], cwd=root, capture_output=True, text=True,
-                       timeout=600)
+                       timeout=600, env=dict(os.environ, **env))
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
     assert "all cases passed" in r.stdout
