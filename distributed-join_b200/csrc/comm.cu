@@ -14,13 +14,29 @@
 
 #include <algorithm>
 #include <chrono>
+#include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
+#include <mutex>
 #include <vector>
 
 #include "dj_device.cuh"
 #include "dj_internal.h"
+
+// In-process rank group (dj_comm_create_local_group): the host-side meeting point that replaces
+// NCCL's control collectives when every rank is a thread of one process on one device.
+struct LocalGroup {
+  explicit LocalGroup(int n) : size(n), here(n, 0), in(n), out(n) {}
+  int size;
+  std::mutex mu;
+  std::condition_variable cv;
+  uint64_t gen = 0;  // completed all-gathers
+  int arrived  = 0;
+  std::vector<char> here;                   // [size] arrived in the current generation
+  std::vector<std::vector<int64_t>> in, out;  // [size] words being gathered / of the last generation
+};
 
 struct dj_comm {
   ncclComm_t nccl = nullptr;
@@ -58,6 +74,9 @@ struct dj_comm {
   int64_t* h_pinned = nullptr;  // pinned scratch
   int64_t* d_small  = nullptr;  // device scratch for tiny collectives
   size_t small_elems = 0;
+  // Set on the members of an in-process group: control all-gathers meet here instead of in NCCL,
+  // peer memory is the siblings' own allocations, and nothing synchronises the whole device.
+  std::shared_ptr<LocalGroup> group;
 };
 
 namespace dj {
@@ -95,6 +114,7 @@ static int ensure_events(dj_comm* c, int n)
 using namespace dj;
 
 static int ctrl_allgather(dj_comm* c, const int64_t* h_mine, int n, int64_t* h_all);
+static int create_streams_and_scratch(dj_comm* c);
 
 static int ensure_xevents(dj_comm* c, int n)
 {
@@ -106,6 +126,50 @@ static int ensure_xevents(dj_comm* c, int n)
     c->ev_xend.push_back(b);
   }
   return DJ_OK;
+}
+
+// Control all-gather of a local group: each rank's thread deposits its words, the last one to
+// arrive publishes the generation.  The wait is bounded so that a rank that never arrives (an
+// exception in its thread, a mismatched call sequence) turns into an error, not a hang.
+constexpr int kGroupTimeoutS = 120;
+
+static int group_allgather(dj_comm* c, const int64_t* h_mine, int n, int64_t* h_all)
+{
+  LocalGroup& g = *c->group;
+  std::unique_lock<std::mutex> lk(g.mu);
+  const uint64_t gen = g.gen;
+  g.in[c->rank].assign(h_mine, h_mine + n);
+  g.here[c->rank] = 1;
+  if (++g.arrived == g.size) {
+    // `out` of the previous generation is no longer read: every rank has arrived again since
+    g.out.swap(g.in);
+    g.arrived = 0;
+    std::fill(g.here.begin(), g.here.end(), 0);
+    g.gen++;
+    g.cv.notify_all();
+  } else if (!g.cv.wait_for(lk, std::chrono::seconds(kGroupTimeoutS), [&] { return g.gen != gen; })) {
+    int missing = 0;
+    while (missing < g.size && g.here[missing]) missing++;
+    set_error("local group: rank %d waited %d s at a collective that rank %d never joined", c->rank, kGroupTimeoutS,
+              missing);
+    return DJ_ERR_NCCL;
+  }
+  for (int r = 0; r < g.size; r++) {
+    DJ_REQUIRE(g.out[r].size() == (size_t)n, "local group: rank %d gathered %d words, rank %d sent %zu", c->rank, n, r,
+               g.out[r].size());
+    memcpy(h_all + (size_t)r * n, g.out[r].data(), (size_t)n * 8);
+  }
+  return DJ_OK;
+}
+
+// What a local-group rank waits for instead of cudaDeviceSynchronize: a device-wide wait from one
+// rank's thread would also wait for a sibling's stream parked on a flag this thread has yet to raise.
+static void sync_own_streams(dj_comm* c)
+{
+  for (cudaStream_t s : {c->comm_stream, c->ctrl_stream})
+    if (s) cudaStreamSynchronize(s);
+  for (auto ps : c->peer_stream)
+    if (ps) cudaStreamSynchronize(ps);
 }
 
 // The stream waits until *d_flag >= value (a peer raises it over NVLink).
@@ -181,11 +245,17 @@ __global__ void verdict_kernel(const unsigned long long* d_count, unsigned long 
   }
 }
 
-// Maps every peer's flag block; decides (collectively) whether the copy-engine exchange is usable.
-static int setup_peer_exchange(dj_comm* c)
+static bool exchange_forced_to_nccl()
 {
   const char* mode = getenv("DJ_EXCHANGE");
-  bool ok = !(mode && (mode[0] == 'n' || mode[0] == 'N'));  // DJ_EXCHANGE=nccl forces the NCCL path
+  return mode && (mode[0] == 'n' || mode[0] == 'N');
+}
+
+// The stream memory operations' driver entry points, and this rank's flag block + control inbox
+// (zeroed).  *entry_ok: every entry point was found.
+static int alloc_ctrl_block(dj_comm* c, bool* entry_ok)
+{
+  bool ok = true;
   cudaDriverEntryPointQueryResult q;
   void* fn = nullptr;
   if (cudaGetDriverEntryPoint("cuStreamWaitValue32", &fn, cudaEnableDefault, &q) != cudaSuccess || !fn) ok = false;
@@ -197,12 +267,24 @@ static int setup_peer_exchange(dj_comm* c)
   if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess || !fn) ok = false;
   c->fn_addr_range = (decltype(c->fn_addr_range))fn;
   cudaGetLastError();
+  *entry_ok = ok;
 
   const size_t flag_bytes = align_up((size_t)c->size * kFlagSlots * sizeof(uint32_t), 256);
   const size_t ctl_bytes  = flag_bytes + (size_t)kInboxBanks * c->size * kInbox * sizeof(int64_t);
   DJ_CUDA_TRY(cudaMalloc(&c->d_flags, ctl_bytes));
   DJ_CUDA_TRY(cudaMemset(c->d_flags, 0, ctl_bytes));
   c->d_inbox = reinterpret_cast<int64_t*>(reinterpret_cast<char*>(c->d_flags) + flag_bytes);
+  return DJ_OK;
+}
+
+// Maps every peer's flag block; decides (collectively) whether the copy-engine exchange is usable.
+static int setup_peer_exchange(dj_comm* c)
+{
+  bool ok = !exchange_forced_to_nccl(), entry_ok = false;
+  int rc = alloc_ctrl_block(c, &entry_ok);
+  if (rc) return rc;
+  ok = ok && entry_ok;
+  const size_t flag_bytes = align_up((size_t)c->size * kFlagSlots * sizeof(uint32_t), 256);
   cudaIpcMemHandle_t mine;
   if (cudaIpcGetMemHandle(&mine, c->d_flags) != cudaSuccess) {
     ok = false;
@@ -213,7 +295,7 @@ static int setup_peer_exchange(dj_comm* c)
   std::vector<int64_t> send(9), all((size_t)c->size * 9);
   send[0] = ok ? 1 : 0;
   memcpy(&send[1], &mine, 64);
-  int rc = ctrl_allgather(c, send.data(), 9, all.data());
+  rc = ctrl_allgather(c, send.data(), 9, all.data());
   if (rc) return rc;
   for (int r = 0; r < c->size; r++) ok = ok && all[(size_t)r * 9] == 1;
   c->peer_flags.assign(c->size, nullptr);
@@ -255,6 +337,8 @@ static int setup_peer_exchange(dj_comm* c)
 }
 
 // Peer view of rank `peer`'s workspace allocation described by (handle, offset); opened once.
+// In a local group the "handle" is the peer's raw workspace pointer: the cache still runs, but
+// nothing is opened or closed.
 static char* map_peer_workspace(dj_comm* c, int peer, const cudaIpcMemHandle_t& h, int64_t offset)
 {
   auto& cache = c->ipc_cache[peer];
@@ -268,11 +352,13 @@ static char* map_peer_workspace(dj_comm* c, int peer, const cudaIpcMemHandle_t& 
   // a peer rarely alternates between more than two live workspaces: older mappings are closed so
   // that the memory behind them can really be released by its owner
   while (cache.size() >= 2) {
-    cudaIpcCloseMemHandle(cache.front().base);
+    if (!c->group) cudaIpcCloseMemHandle(cache.front().base);
     cache.erase(cache.begin());
   }
   void* p = nullptr;
-  if (cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
+  if (c->group) {
+    memcpy(&p, &h, sizeof(p));
+  } else if (cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
     cudaGetLastError();
     return nullptr;
   }
@@ -303,6 +389,81 @@ extern "C" int dj_comm_create(int rank, int size, const void* h_id128, dj_comm_t
     DJ_NCCL_TRY(ncclCommInitRank(&c->nccl, size, id, rank));
     DJ_NCCL_TRY(ncclCommSplit(c->nccl, 0, rank, &c->nccl_ctrl, nullptr));
   }
+  int rc = create_streams_and_scratch(c);
+  if (rc) return rc;
+  if (size > 1) {
+    rc = setup_peer_exchange(c);
+    if (rc) return rc;
+  }
+  *out           = c;
+  return DJ_OK;
+}
+
+extern "C" int dj_comm_create_local_group(int size, dj_comm_t** comms)
+{
+  DJ_REQUIRE(comms && size >= 1, "comm_create_local_group: bad size");
+  if (size == 1) return dj_comm_create(0, 1, nullptr, comms);
+  // Every rank queues work on size + 2 streams of one context.  When they share fewer hardware
+  // queues, a stream parked on a peer's flag can hold up the write that would raise it.
+  const char* e   = getenv("CUDA_DEVICE_MAX_CONNECTIONS");
+  const int conns = e && atoi(e) > 0 ? atoi(e) : 8;
+  DJ_REQUIRE(size * (size + 2) <= conns,
+             "comm_create_local_group: %d ranks use %d streams, more than CUDA_DEVICE_MAX_CONNECTIONS = %d hardware "
+             "queues (set it, up to 32, before CUDA starts)", size, size * (size + 2), conns);
+  DJ_REQUIRE(!exchange_forced_to_nccl(), "comm_create_local_group: DJ_EXCHANGE=nccl needs NCCL, which a local group "
+             "does not have");
+  auto g = std::make_shared<LocalGroup>(size);
+  std::vector<dj_comm*> cs(size, nullptr);
+  auto fail = [&](int rc) {
+    for (auto c : cs) dj_comm_destroy(c);
+    for (int r = 0; r < size; r++) comms[r] = nullptr;
+    return rc;
+  };
+  bool entry_ok = true;
+  for (int r = 0; r < size; r++) {
+    dj_comm* c = cs[r] = new dj_comm();
+    c->rank = r;
+    c->size = size;
+    c->group = g;
+    int rc = cudaGetDevice(&c->device) == cudaSuccess ? create_streams_and_scratch(c) : DJ_ERR_CUDA;
+    bool ok = false;
+    if (!rc) rc = alloc_ctrl_block(c, &ok);
+    if (rc) return fail(rc);
+    entry_ok = entry_ok && ok;
+  }
+  if (!entry_ok) {
+    set_error("comm_create_local_group: the driver lacks the stream memory operations the exchange needs");
+    return fail(DJ_ERR_CUDA);
+  }
+  // peer memory: the siblings' own flag blocks and inboxes, no mapping
+  for (int r = 0; r < size; r++) {
+    dj_comm* c = cs[r];
+    c->peer_flags.assign(size, nullptr);
+    c->peer_inbox.assign(size, nullptr);
+    c->peer_stream.assign(size, nullptr);
+    c->ipc_cache.assign(size, {});
+    for (int p = 0; p < size; p++) {
+      c->peer_flags[p] = cs[p]->d_flags;
+      c->peer_inbox[p] = cs[p]->d_inbox;
+      if (p != r && cudaStreamCreateWithFlags(&c->peer_stream[p], cudaStreamNonBlocking) != cudaSuccess) {
+        set_error("comm_create_local_group: cudaStreamCreate failed");
+        return fail(DJ_ERR_CUDA);
+      }
+    }
+    if (cudaMalloc(&c->d_peer_flags, (size_t)size * sizeof(uint32_t*)) != cudaSuccess ||
+        cudaMemcpy(c->d_peer_flags, c->peer_flags.data(), (size_t)size * sizeof(uint32_t*), cudaMemcpyHostToDevice) !=
+          cudaSuccess) {
+      set_error("comm_create_local_group: cannot allocate the peer flag table");
+      return fail(DJ_ERR_CUDA);
+    }
+    c->peer_ok = true;
+  }
+  for (int r = 0; r < size; r++) comms[r] = cs[r];
+  return DJ_OK;
+}
+
+static int create_streams_and_scratch(dj_comm* c)
+{
   DJ_CUDA_TRY(cudaStreamCreateWithFlags(&c->comm_stream, cudaStreamNonBlocking));
   DJ_CUDA_TRY(cudaStreamCreateWithFlags(&c->ctrl_stream, cudaStreamNonBlocking));
   DJ_CUDA_TRY(cudaEventCreateWithFlags(&c->ev_ready, cudaEventDisableTiming));
@@ -314,18 +475,16 @@ extern "C" int dj_comm_create(int rank, int size, const void* h_id128, dj_comm_t
   DJ_CUDA_TRY(cudaMallocHost(&c->h_pinned, kSmallElems * sizeof(int64_t)));
   DJ_CUDA_TRY(cudaMalloc(&c->d_small, kSmallElems * sizeof(int64_t)));
   c->small_elems = kSmallElems;
-  if (size > 1) {
-    int rc = setup_peer_exchange(c);
-    if (rc) return rc;
-  }
-  *out           = c;
   return DJ_OK;
 }
 
 extern "C" int dj_comm_destroy(dj_comm_t* c)
 {
   if (!c) return DJ_OK;
-  cudaDeviceSynchronize();
+  if (c->group)
+    sync_own_streams(c);
+  else
+    cudaDeviceSynchronize();
   if (c->nccl_ctrl) ncclCommDestroy(c->nccl_ctrl);
   if (c->nccl) ncclCommDestroy(c->nccl);
   for (int i = 0; i < 2; i++) {
@@ -335,10 +494,11 @@ extern "C" int dj_comm_destroy(dj_comm_t* c)
   if (c->ctrl_stream) cudaStreamDestroy(c->ctrl_stream);
   for (auto ps : c->peer_stream)
     if (ps) cudaStreamDestroy(ps);
-  for (int i = 0; i < (int)c->peer_flags.size(); i++)
+  for (int i = 0; i < (int)c->peer_flags.size() && !c->group; i++)
     if (c->peer_flags[i] && i != c->rank) cudaIpcCloseMemHandle(c->peer_flags[i]);
   for (auto& v : c->ipc_cache)
-    for (auto& e : v) cudaIpcCloseMemHandle(e.base);
+    for (auto& e : v)
+      if (!c->group) cudaIpcCloseMemHandle(e.base);
   if (c->d_flags) cudaFree(c->d_flags);
   if (c->d_peer_flags) cudaFree(c->d_peer_flags);
   for (auto e : c->ev_xbeg) cudaEventDestroy(e);
@@ -359,9 +519,13 @@ extern "C" int dj_comm_destroy(dj_comm_t* c)
 extern "C" int dj_comm_release_workspace(dj_comm_t* c)
 {
   if (!c || c->size == 1) return DJ_OK;
-  cudaDeviceSynchronize();
+  if (c->group)
+    sync_own_streams(c);
+  else
+    cudaDeviceSynchronize();
   for (auto& v : c->ipc_cache) {
-    for (auto& e : v) cudaIpcCloseMemHandle(e.base);
+    for (auto& e : v)
+      if (!c->group) cudaIpcCloseMemHandle(e.base);
     v.clear();
   }
   c->last_handle.clear();
@@ -385,6 +549,10 @@ extern "C" int dj_comm_allgather_i64(dj_comm_t* c, const int64_t* h_mine, int n,
   }
   DJ_REQUIRE((size_t)n * (c->size + 1) <= c->small_elems, "allgather: %d values per rank is too many", n);
   cudaStream_t st = (cudaStream_t)stream;
+  if (c->group) {  // same ordering as the NCCL path: the stream's earlier work is done on return
+    DJ_CUDA_TRY(cudaStreamSynchronize(st));
+    return group_allgather(c, h_mine, n, h_all);
+  }
   int64_t* d_send = c->d_small;
   int64_t* d_recv = c->d_small + n;
   memcpy(c->h_pinned, h_mine, (size_t)n * 8);
@@ -404,6 +572,7 @@ static int ctrl_allgather(dj_comm* c, const int64_t* h_mine, int n, int64_t* h_a
     memcpy(h_all, h_mine, (size_t)n * 8);
     return DJ_OK;
   }
+  if (c->group) return group_allgather(c, h_mine, n, h_all);
   const size_t half = c->small_elems / 2;  // second half of both scratch areas
   DJ_REQUIRE((size_t)n * (c->size + 1) <= half / 4, "allgather: %d values per rank is too many", n);
   cudaStream_t st = c->ctrl_stream;
@@ -438,25 +607,27 @@ extern "C" int dj_comm_barrier(dj_comm_t* c, void* stream)
   return dj_comm_allgather_i64(c, &mine, 1, all.data(), stream);
 }
 
-extern "C" int dj_comm_group_start(dj_comm_t*)
+extern "C" int dj_comm_group_start(dj_comm_t* c)
 {
+  DJ_REQUIRE(!c || !c->group, "group_start: a local group has no NCCL");
   DJ_NCCL_TRY(ncclGroupStart());
   return DJ_OK;
 }
-extern "C" int dj_comm_group_end(dj_comm_t*)
+extern "C" int dj_comm_group_end(dj_comm_t* c)
 {
+  DJ_REQUIRE(!c || !c->group, "group_end: a local group has no NCCL");
   DJ_NCCL_TRY(ncclGroupEnd());
   return DJ_OK;
 }
 extern "C" int dj_comm_send(dj_comm_t* c, const void* d_buf, int64_t nbytes, int dest, void* stream)
 {
-  DJ_REQUIRE(c && c->nccl, "send: communicator has no NCCL (size 1)");
+  DJ_REQUIRE(c && c->nccl, "send: communicator has no NCCL (size 1 or a local group)");
   DJ_NCCL_TRY(ncclSend(d_buf, (size_t)nbytes, ncclInt8, dest, c->nccl, (cudaStream_t)stream));
   return DJ_OK;
 }
 extern "C" int dj_comm_recv(dj_comm_t* c, void* d_buf, int64_t nbytes, int source, void* stream)
 {
-  DJ_REQUIRE(c && c->nccl, "recv: communicator has no NCCL (size 1)");
+  DJ_REQUIRE(c && c->nccl, "recv: communicator has no NCCL (size 1 or a local group)");
   DJ_NCCL_TRY(ncclRecv(d_buf, (size_t)nbytes, ncclInt8, source, c->nccl, (cudaStream_t)stream));
   return DJ_OK;
 }
@@ -468,6 +639,7 @@ extern "C" int dj_all_to_all(dj_comm_t* c, int group_size, const int* h_group_ra
 {
   DJ_REQUIRE(c && group_size >= 1 && self_idx >= 0 && self_idx < group_size && ncols >= 0,
              "all_to_all: bad argument");
+  DJ_REQUIRE(group_size == 1 || c->nccl, "all_to_all: communicator has no NCCL (size 1 or a local group)");
   cudaStream_t st = (cudaStream_t)stream;
   if (include_self) {
     const int64_t n = h_send_offsets[self_idx + 1] - h_send_offsets[self_idx];
@@ -481,7 +653,6 @@ extern "C" int dj_all_to_all(dj_comm_t* c, int group_size, const int* h_group_ra
     }
   }
   if (group_size == 1) return DJ_OK;
-  DJ_REQUIRE(c->nccl, "all_to_all: communicator has no NCCL (size 1)");
   DJ_NCCL_TRY(ncclGroupStart());
   for (int col = 0; col < ncols; col++) {
     const size_t es = (size_t)h_elem_sizes[col];
@@ -578,9 +749,9 @@ struct Trace {
   void dump(int rank)
   {
     if (!on) return;
-    cudaDeviceSynchronize();
-    for (auto& m : marks) {
+    for (auto& m : marks) {  // the marks' own events: a device-wide sync could wait on a sibling rank's stream
       float ms = 0;
+      cudaEventSynchronize(m.second);
       cudaEventElapsedTime(&ms, base, m.second);
       printf("[trace rank %d] %8.3f ms  %s\n", rank, ms, m.first);
       cudaEventDestroy(m.second);
@@ -678,7 +849,11 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
   std::vector<int64_t> hello((size_t)world * kHello);
   {
     int64_t mine[kHello] = {nleft, nright, (int64_t)workspace_bytes, 0, 0};
-    if (comm->peer_ok) {
+    if (comm->peer_ok && comm->group) {
+      // one address space: the raw workspace pointer stands in for the IPC handle (offset 0)
+      mine[3] = 1;
+      memcpy(&mine[5], &d_workspace, sizeof(d_workspace));
+    } else if (comm->peer_ok) {
       CUdeviceptr base = 0;
       size_t alloc_sz  = 0;
       cudaIpcMemHandle_t wh;
@@ -811,6 +986,12 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
       set_error("distributed_inner_join: a cached peer mapping disappeared");
       return DJ_ERR_CUDA;
     }
+  }
+  if (!use_peer && !comm->nccl) {  // identical on every rank: nothing has been queued but the count reset
+    set_error("distributed_inner_join: this exchange (odf %d; peer memory carries at most %d) needs NCCL, which a "
+              "local group does not have", odf, kDataSlots / 2);
+    cudaStreamSynchronize(st);
+    return DJ_ERR_ARG;
   }
   trace.host("peer workspaces mapped");
   const uint32_t seq = use_peer ? ++comm->seq : 0;
@@ -1461,7 +1642,9 @@ extern "C" int dj_distributed_inner_join_i64_host(
   int64_t* o[4];
   for (int c = 0; c < 4; c++) o[c] = arena.take<int64_t>((size_t)out_capacity);
   if (!dlk || !dlp || !drk || !drp || !o[0] || !o[1] || !o[2] || !o[3]) {
-    set_error("distributed_inner_join_host: workspace too small");
+    // unlike the join's own verdict this one is local: size the workspace with
+    // dj_distributed_inner_join_host_workspace_bytes, which always leaves room for the staging
+    set_error("distributed_inner_join_host: workspace too small for the staged columns");
     return DJ_ERR_WORKSPACE;
   }
   DJ_CUDA_TRY(cudaMemcpyAsync(dlk, h_left_key, (size_t)nleft * 8, cudaMemcpyHostToDevice, st));
@@ -1472,6 +1655,8 @@ extern "C" int dj_distributed_inner_join_i64_host(
   int rc = dj_distributed_inner_join_i64(comm, dlk, dlp, nleft, drk, drp, nright, o[0], o[1], o[2],
                                          o[3], out_capacity, h_out_count, opts,
                                          (char*)d_workspace + off, workspace_bytes - off, stream);
+  // the device join sized only what follows the staged columns: report the whole workspace
+  if (rc == DJ_ERR_WORKSPACE && opts && opts->workspace_needed > 0) opts->workspace_needed += (int64_t)off;
   if (rc && rc != DJ_ERR_OVERFLOW) return rc;
   const int64_t n = *h_out_count < out_capacity ? *h_out_count : out_capacity;
   for (int c = 0; c < 4; c++)

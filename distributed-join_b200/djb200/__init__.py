@@ -71,7 +71,7 @@ ABI_SYMBOLS = [
     "dj_comm_allgather_i64", "dj_comm_barrier", "dj_all_to_all", "dj_comm_group_start",
     "dj_comm_group_end", "dj_comm_send", "dj_comm_recv", "dj_distributed_inner_join_workspace_bytes",
     "dj_distributed_inner_join_i64", "dj_distributed_inner_join_host_workspace_bytes",
-    "dj_distributed_inner_join_i64_host",
+    "dj_distributed_inner_join_i64_host", "dj_comm_create_local_group",
 ]
 
 _lib = None
@@ -124,6 +124,7 @@ def lib() -> C.CDLL:
     L.dj_distributed_inner_join_host_workspace_bytes.restype = sz
     L.dj_distributed_inner_join_host_workspace_bytes.argtypes = [i64, i64, i64, C.c_int, C.c_int]
     L.dj_distributed_inner_join_i64_host.argtypes = L.dj_distributed_inner_join_i64.argtypes
+    L.dj_comm_create_local_group.argtypes = [C.c_int, C.POINTER(vp)]
     _lib = L
     return L
 
@@ -307,6 +308,19 @@ class Comm:
         dist.broadcast(idt, 0)
         return cls(rank, size, bytes(idt.cpu().tolist()))
 
+    @classmethod
+    def local_group(cls, n: int) -> list:
+        """`n` communicators (ranks 0..n-1) on the current device in this process, for testing the
+        multi-rank path on one GPU.  Drive each from its own thread (dj_comm_create_local_group)."""
+        handles = (C.c_void_p * n)()
+        _check(lib().dj_comm_create_local_group(n, handles))
+        comms = []
+        for r in range(n):
+            c = cls.__new__(cls)
+            c.rank, c.size, c.handle = r, n, C.c_void_p(handles[r])
+            comms.append(c)
+        return comms
+
     def allgather_i64(self, values):
         n = len(values)
         mine = (C.c_int64 * n)(*values)
@@ -365,23 +379,40 @@ def distributed_inner_join(comm, lk, lp, rk, rp, odf=1, capacity=None, ws=None, 
             comm.release_workspace()
             need = int(opts.workspace_needed)
             ws = workspace(max(ws.numel(), need + need // 8), dev)
+            comm.barrier()  # no rank re-enters the call while a peer is still allocating
             continue
         # every rank must retry together: agree on the largest need
         need = max(comm.allgather_i64([n])) if comm and comm.size > 1 else n
         capacity = need
-        outs = None
+        outs = [torch.empty(capacity, dtype=torch.int64, device=dev) for _ in range(4)]
+        if comm and comm.size > 1:
+            comm.barrier()
 
 
 def distributed_inner_join_host(comm, h_lk, h_lp, h_rk, h_rp, h_outs, odf=1, ws=None):
-    """End-to-end entry: HOST (pinned) inputs and outputs, copies inside the call."""
+    """End-to-end entry: HOST (pinned) inputs and outputs, copies inside the call.  A workspace that
+    is too small on any rank is grown and the call retried on every rank, as in distributed_inner_join;
+    the host outputs belong to the caller, so an overflow raises (on every rank)."""
     nl, nr = h_lk.numel(), h_rk.numel()
     capacity = h_outs[0].numel()
     world = comm.size if comm else 1
     if ws is None:
         ws = workspace(lib().dj_distributed_inner_join_host_workspace_bytes(nl, nr, capacity, world, odf))
-    cnt = C.c_int64(0)
-    opts = JoinOptions(odf, 0, 0, 0, 0, 0)
-    _check(lib().dj_distributed_inner_join_i64_host(comm.handle if comm else None, _ptr(h_lk), _ptr(h_lp), nl,
-                                                    _ptr(h_rk), _ptr(h_rp), nr, *[_ptr(o) for o in h_outs], capacity,
-                                                    C.byref(cnt), C.byref(opts), _ptr(ws), ws.numel(), _stream()))
-    return cnt.value, opts
+    while True:
+        cnt = C.c_int64(0)
+        opts = JoinOptions(odf, 0, 0, 0, 0, 0)
+        rc = _check(lib().dj_distributed_inner_join_i64_host(comm.handle if comm else None, _ptr(h_lk), _ptr(h_lp),
+                                                             nl, _ptr(h_rk), _ptr(h_rp), nr,
+                                                             *[_ptr(o) for o in h_outs], capacity, C.byref(cnt),
+                                                             C.byref(opts), _ptr(ws), ws.numel(), _stream()),
+                    allow=(ERR_WORKSPACE,) if world > 1 else ())
+        if rc == 0:
+            return cnt.value, opts
+        comm.release_workspace()
+        need = int(opts.workspace_needed)
+        # collective: a retry that no rank's workspace grows for would fail the same way forever
+        if not any(comm.allgather_i64([1 if need > ws.numel() else 0])):
+            raise DjError(f"distributed_inner_join_host: no rank needs a larger workspace, yet rank {comm.rank} "
+                          f"got DJ_ERR_WORKSPACE: {lib().dj_last_error().decode()}")
+        ws = workspace(max(ws.numel(), need + need // 8))
+        comm.barrier()

@@ -40,7 +40,7 @@ enum {
   DJ_ERR_CUDA      = 1, /* a CUDA runtime call or kernel launch failed              */
   DJ_ERR_ARG       = 2, /* invalid argument (the reference throws std::runtime_error) */
   DJ_ERR_WORKSPACE = 3, /* workspace too small                                        */
-  DJ_ERR_NCCL      = 4, /* an NCCL call failed                                        */
+  DJ_ERR_NCCL      = 4, /* an NCCL call failed, or a local group's collective timed out */
   DJ_ERR_OVERFLOW  = 5  /* output capacity too small (count is still exact)           */
 };
 
@@ -215,7 +215,8 @@ int dj_distributed_inner_join_i64(dj_comm_t* comm,
 
 /* Same join with HOST input/output buffers (pinned recommended): the end-to-end entry
  * bench.py times.  Copies inputs host->device, runs the device path above, copies the
- * result columns device->host.  Device memory is taken from d_workspace. */
+ * result columns device->host.  Device memory is taken from d_workspace; with
+ * DJ_ERR_WORKSPACE, opts->workspace_needed counts the staged columns too. */
 size_t dj_distributed_inner_join_host_workspace_bytes(int64_t nleft, int64_t nright,
                                                       int64_t out_capacity, int world,
                                                       int over_decom_factor);
@@ -228,6 +229,23 @@ int dj_distributed_inner_join_i64_host(dj_comm_t* comm,
                                        int64_t* h_out_rp, int64_t out_capacity,
                                        int64_t* h_out_count, dj_join_options* opts,
                                        void* d_workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------
+ * Testing: an in-process rank group.  Creates `size` communicators (ranks 0..size-1) on the
+ * current device in one process; comms[r] is meant to be driven by its own host thread.  The
+ * multi-rank join runs unchanged from its first control message to its overflow verdict; only
+ * what needs NCCL or cross-process IPC is replaced: control all-gathers meet in host memory
+ * (bounded wait: a rank that does not arrive within 120 s fails the others' call with
+ * DJ_ERR_NCCL), and peer memory is the siblings' own allocations.  NCCL entry points
+ * (send/recv/group calls, dj_all_to_all across ranks, DJ_EXCHANGE=nccl, and the join's NCCL
+ * fallback for over_decom_factor > 31) return an error.  Each rank queues work on size + 2
+ * streams, so size * (size + 2) must not exceed CUDA_DEVICE_MAX_CONNECTIONS (default 8, at
+ * most 32; set it before CUDA starts).  Threads driving a group must not synchronise the
+ * whole device (cudaDeviceSynchronize, cudaFree) while a sibling is inside a call: the
+ * sibling's streams may be waiting for a flag that only this thread's next call raises.
+ * Destroy every member with dj_comm_destroy once no thread is inside a call.
+ */
+int dj_comm_create_local_group(int size, dj_comm_t** comms);
 
 #if defined(DJ_BUILDING) && defined(__GNUC__)
 #pragma GCC visibility pop

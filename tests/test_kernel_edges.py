@@ -56,6 +56,25 @@ def plan_bits(nbuild):
     return sum(plan_split(nbuild))
 
 
+MAX_FANOUT = 1024  # dj_internal.h kMaxFanout
+
+
+def dist_plan(tot_left, tot_right, world, odf, no_fuse=False):
+    """(bits1, bits2, sub_bits) of the multi-rank join (comm.cu, after the hello): the plan for the
+    estimated build rows per rank and batch; a two-level plan moves up to `fit` level-1 bits into the
+    sender's partition (sub_bits) when the rest still fits one level of at most 10 bits."""
+    nparts = world * odf
+    bits1, bits2 = plan_split(min(tot_left, tot_right) // nparts + 1)
+    fit = 0  # largest sub_bits with nparts << sub_bits <= MAX_FANOUT
+    while (nparts << (fit + 1)) <= MAX_FANOUT:
+        fit += 1
+    if bits2 > 0 and fit > 0 and not no_fuse:
+        b1 = min(bits1, fit)
+        if bits1 + bits2 - b1 <= 10:
+            return b1, bits1 + bits2 - b1, b1
+    return bits1, bits2, 0
+
+
 def host_chunks(nprobe):
     """(chunk rows, chunk count) of the streamed host entry (comm.cu streamed_shape)."""
     n = int(os.environ.get("DJ_HOST_CHUNKS", "0") or 0)
