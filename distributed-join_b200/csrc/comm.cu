@@ -245,6 +245,61 @@ __global__ void verdict_kernel(const unsigned long long* d_count, unsigned long 
   }
 }
 
+// Loads the code of every kernel of the library (and the CUB kernels instantiated with it) now.
+// Under lazy module loading (CUDA_MODULE_LOADING=LAZY, which PyTorch sets by default) a kernel is
+// loaded at its first launch, and the driver may synchronise the whole context to do it.  The
+// ranks of a local group share one context: a rank whose stream is parked on a peer's flag then
+// holds up the load of a kernel that peer must run before it raises that flag, and neither rank
+// moves again, so a group's first join could hang (it is the first launch of most kernels).  Loading everything up
+// front, before any rank can wait, removes the load from the ranks' paths.
+static int load_all_kernels()
+{
+  static std::mutex mu;
+  static bool done = false;
+  std::lock_guard<std::mutex> lock(mu);
+  if (done) return DJ_OK;
+  cudaDriverEntryPointQueryResult q;
+  void* fn = nullptr;
+  CUmoduleLoadingMode mode = CU_MODULE_LAZY_LOADING;
+  if (cudaGetDriverEntryPoint("cuModuleGetLoadingMode", &fn, cudaEnableDefault, &q) == cudaSuccess && fn &&
+      ((CUresult(*)(CUmoduleLoadingMode*))fn)(&mode) == CUDA_SUCCESS && mode == CU_MODULE_EAGER_LOADING) {
+    done = true;
+    return DJ_OK;
+  }
+  void *get_module = nullptr, *count = nullptr, *enumerate = nullptr, *load = nullptr;
+  const bool found = cudaGetDriverEntryPoint("cuFuncGetModule", &get_module, cudaEnableDefault, &q) == cudaSuccess &&
+                     cudaGetDriverEntryPoint("cuModuleGetFunctionCount", &count, cudaEnableDefault, &q) == cudaSuccess &&
+                     cudaGetDriverEntryPoint("cuModuleEnumerateFunctions", &enumerate, cudaEnableDefault, &q) ==
+                       cudaSuccess &&
+                     cudaGetDriverEntryPoint("cuFuncLoad", &load, cudaEnableDefault, &q) == cudaSuccess && get_module &&
+                     count && enumerate && load;
+  cudaGetLastError();
+  if (!found) {
+    set_error("the driver cannot load the library's kernels ahead of use (CUDA 12.4 or newer needed); "
+              "set CUDA_MODULE_LOADING=EAGER before CUDA starts");
+    return DJ_ERR_CUDA;
+  }
+  const void* anchors[] = {(const void*)verdict_kernel, dj::partition_module_kernel(), dj::join_module_kernel(),
+                           dj::generate_module_kernel()};
+  for (const void* a : anchors) {
+    cudaFunction_t f = nullptr;
+    DJ_CUDA_TRY(cudaGetFuncBySymbol(&f, a));
+    CUmodule m = nullptr;
+    unsigned n = 0;
+    bool ok = ((CUresult(*)(CUmodule*, CUfunction))get_module)(&m, (CUfunction)f) == CUDA_SUCCESS &&
+              ((CUresult(*)(unsigned*, CUmodule))count)(&n, m) == CUDA_SUCCESS;
+    std::vector<CUfunction> fs(n);
+    ok = ok && (n == 0 || ((CUresult(*)(CUfunction*, unsigned, CUmodule))enumerate)(fs.data(), n, m) == CUDA_SUCCESS);
+    for (unsigned i = 0; ok && i < n; i++) ok = ((CUresult(*)(CUfunction))load)(fs[i]) == CUDA_SUCCESS;
+    if (!ok) {
+      set_error("cannot load the library's kernels ahead of use; set CUDA_MODULE_LOADING=EAGER before CUDA starts");
+      return DJ_ERR_CUDA;
+    }
+  }
+  done = true;
+  return DJ_OK;
+}
+
 static bool exchange_forced_to_nccl()
 {
   const char* mode = getenv("DJ_EXCHANGE");
@@ -392,6 +447,8 @@ extern "C" int dj_comm_create(int rank, int size, const void* h_id128, dj_comm_t
   int rc = create_streams_and_scratch(c);
   if (rc) return rc;
   if (size > 1) {
+    rc = load_all_kernels();  // this rank's own streams also park on peer flags
+    if (rc) return rc;
     rc = setup_peer_exchange(c);
     if (rc) return rc;
   }
@@ -412,6 +469,7 @@ extern "C" int dj_comm_create_local_group(int size, dj_comm_t** comms)
              "queues (set it, up to 32, before CUDA starts)", size, size * (size + 2), conns);
   DJ_REQUIRE(!exchange_forced_to_nccl(), "comm_create_local_group: DJ_EXCHANGE=nccl needs NCCL, which a local group "
              "does not have");
+  if (int rc = load_all_kernels()) return rc;
   auto g = std::make_shared<LocalGroup>(size);
   std::vector<dj_comm*> cs(size, nullptr);
   auto fail = [&](int rc) {

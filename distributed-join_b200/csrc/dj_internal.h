@@ -180,4 +180,10 @@ int local_join(const int64_t* bk, const int64_t* bp, int64_t nb, const int64_t* 
                int64_t* d_out_count, bool swap, Arena& arena, cudaStream_t stream);
 size_t local_join_workspace(int64_t nb, int64_t np);
 
+// One kernel of each translation unit's module (partition.cu, join.cu, generate.cu): comm.cu
+// loads every function of these modules before ranks can wait on each other.
+const void* partition_module_kernel();
+const void* join_module_kernel();
+const void* generate_module_kernel();
+
 }  // namespace dj

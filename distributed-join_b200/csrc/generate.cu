@@ -159,6 +159,9 @@ int grid_for(int64_t n, int threads)
 }
 
 }  // namespace
+
+const void* generate_module_kernel() { return (const void*)checksum_kernel; }
+
 }  // namespace dj
 
 using namespace dj;

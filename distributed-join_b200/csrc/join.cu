@@ -383,4 +383,6 @@ int run_bucket_join(const JoinBuffers& jb, bool swap_output_sides, cudaStream_t 
   return join_shape() == 1 ? launch_join<CfgB>(d, 2, stream) : launch_join<CfgA>(d, 1, stream);
 }
 
+const void* join_module_kernel() { return (const void*)bucket_join_kernel<CfgA>; }
+
 }  // namespace dj

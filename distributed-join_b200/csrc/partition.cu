@@ -970,4 +970,6 @@ int run_partition_pass(const PassDesc& desc, const PassBuffers& buf, void* d_ws,
   return pass_scatter(st, stream);
 }
 
+const void* partition_module_kernel() { return (const void*)plan_kernel; }
+
 }  // namespace dj

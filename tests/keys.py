@@ -9,6 +9,9 @@ keys_in_bucket  distinct keys whose local hash has the given top bits (one radix
 slot_twins      for each key, a different key with the same 32-bit slot hash in the same bucket,
                 so a probe reaches the build row's slot with a matching fingerprint and only the
                 full key comparison tells them apart.
+mix64, unmix64  the splitmix64 finalizer and its inverse: test payloads are mix64(base + row), so
+                every 32-bit half of a payload word takes full-width values (bit 31 and bit 63
+                set about half the time) while the row stays recoverable with unmix64.
 """
 import numpy as np
 
@@ -16,10 +19,39 @@ _C1 = 0x9E3779B97F4A7C15
 _C2 = 0xD6E8FEB86659FD93
 _C1_INV = pow(_C1, -1, 1 << 64)
 _C2_INV = pow(_C2, -1, 1 << 64)
+_M1 = 0xBF58476D1CE4E5B9  # splitmix64 finalizer multipliers
+_M2 = 0x94D049BB133111EB
+_M1_INV = pow(_M1, -1, 1 << 64)
+_M2_INV = pow(_M2, -1, 1 << 64)
 
 
 def _u64(keys):
     return np.ascontiguousarray(keys, dtype=np.int64).view(np.uint64)
+
+
+def mix64(x) -> np.ndarray:
+    """splitmix64 finalizer on int64 words (uint64 wrap): a bijection of the 64-bit words."""
+    z = _u64(x).copy()
+    with np.errstate(over="ignore"):
+        z ^= z >> np.uint64(30)
+        z *= np.uint64(_M1)
+        z ^= z >> np.uint64(27)
+        z *= np.uint64(_M2)
+        z ^= z >> np.uint64(31)
+    return z.view(np.int64)
+
+
+def unmix64(y) -> np.ndarray:
+    """Inverse of mix64: each xor-shift by s >= 22 is undone by xoring in the shifts by s and 2s,
+    each multiply by the modular inverse."""
+    z = _u64(y).copy()
+    with np.errstate(over="ignore"):
+        z ^= (z >> np.uint64(31)) ^ (z >> np.uint64(62))
+        z *= np.uint64(_M2_INV)
+        z ^= (z >> np.uint64(27)) ^ (z >> np.uint64(54))
+        z *= np.uint64(_M1_INV)
+        z ^= (z >> np.uint64(30)) ^ (z >> np.uint64(60))
+    return z.view(np.int64)
 
 
 def local_hash(keys) -> np.ndarray:

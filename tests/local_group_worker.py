@@ -35,7 +35,8 @@ import torch  # noqa: E402
 import djb200 as dj  # noqa: E402
 import keys as K  # noqa: E402
 import oracle as O  # noqa: E402
-from test_kernel_edges import SORTED_COMPARE_MAX, TARGET, dist_plan  # noqa: E402
+from test_kernel_edges import (BC, GUARD, PC, SENTINEL, SORTED_COMPARE_MAX, TARGET, analytic_count,  # noqa: E402
+                               dist_plan)
 
 W = int(sys.argv[1])
 FUSED = os.environ.get("DJ_EXCHANGE", "")[:1] in ("f", "F")
@@ -83,13 +84,23 @@ def run_ranks(fn):
 
 # ------------------------------------------------------------------------------------------ tables
 def with_payloads(lkeys, rkeys):
-    """Per-rank (lk, lp, rk, rp) with payloads unique over all ranks and both sides."""
+    """Per-rank (lk, lp, rk, rp) with payloads unique over all ranks and both sides: mix64 of
+    (side << 48) + (rank << 36) + row, full-width words that pay_origin decodes."""
     out = []
     for r, (lk, rk) in enumerate(zip(lkeys, rkeys)):
         lk, rk = np.ascontiguousarray(lk, np.int64), np.ascontiguousarray(rk, np.int64)
-        out.append((lk, (r << 36) + np.arange(lk.size, dtype=np.int64), rk,
-                    (1 << 48) + (r << 36) + np.arange(rk.size, dtype=np.int64)))
+        out.append((lk, K.mix64((r << 36) + np.arange(lk.size, dtype=np.int64)), rk,
+                    K.mix64((1 << 48) + (r << 36) + np.arange(rk.size, dtype=np.int64))))
     return out
+
+
+def pay_origin(pay, side):
+    """(source rank, row) of with_payloads payloads of `side` (0 left, 1 right); -1 where the word
+    is no such payload."""
+    u = K.unmix64(pay) - (side << 48)
+    src, row = u >> 36, u & ((1 << 36) - 1)
+    bad = (u < 0) | (src >= W)
+    return np.where(bad, -1, src), np.where(bad, -1, row)
 
 
 def split(a, rng):
@@ -427,6 +438,59 @@ def case_overflow():
     check(tables, 1, [x[3] for x in res], exp, ", retried")
 
 
+def case_count_past_2_31():
+    """Two hot keys owned by each rank, build_chunk left rows x enough right rows each that every
+    rank's count passes 2^31.  At a capacity of 1M rows every rank returns DJ_ERR_OVERFLOW with its
+    exact analytic count; the rows it wrote join equal keys it owns, each payload decodes to a row
+    of its side holding that key, no (left row, right row) pair appears twice, and the guard tail
+    past the capacity keeps its sentinel."""
+    rng = np.random.default_rng([W, 31])
+    pool = keys_pool(256, rng)
+    own = owner(pool, 1)
+    hot = [pool[own == r][:2] for r in range(W)]
+    per_left = BC
+    per_right = -(-(1 << 31) // (2 * per_left)) + PC + 1
+    allhot = np.concatenate(hot)
+    lk = rng.permutation(np.repeat(allhot, per_left))
+    rk = rng.permutation(np.repeat(allhot, per_right))
+    tables = with_payloads(split(lk, rng), split(rk, rng))
+    counts = [analytic_count(lk[np.isin(lk, h)], rk[np.isin(rk, h)]) for h in hot]
+    assert all(c > 1 << 31 for c in counts), counts
+    cap = 1_000_000
+    dev = upload(tables)
+    ws_bytes = dj.lib().dj_distributed_inner_join_workspace_bytes(lk.size, rk.size, W, 1)
+
+    def fn(r, comm, sync):
+        ws = dj.workspace(ws_bytes)
+        outs = [torch.full((cap + GUARD,), SENTINEL, dtype=torch.int64, device="cuda") for _ in range(4)]
+        sync()
+        return raw_join(comm, dev[r], 1, cap, ws, outs), outs
+
+    for r, ((rc, n, _, err), outs) in enumerate(run_ranks(fn)):
+        assert rc == dj.ERR_OVERFLOW, f"rank {r}: rc {rc} ({err})"
+        assert n == counts[r], f"rank {r}: count {n}, analytic {counts[r]}"
+        k0, p0, k2, p2 = [o.cpu().numpy() for o in outs]
+        for c in (k0, p0, k2, p2):
+            assert (c[cap:] == SENTINEL).all(), f"rank {r}: write past the capacity"
+        k0, p0, k2, p2 = k0[:cap], p0[:cap], k2[:cap], p2[:cap]
+        assert (k0 == k2).all() and np.isin(k0, hot[r]).all(), f"rank {r}: a key it does not own or unequal keys"
+        ids = []
+        for side, pay, key in ((0, p0, k0), (1, p2, k2)):
+            src, row = pay_origin(pay, side)
+            assert (src >= 0).all(), f"rank {r}: side {side} payload that no row carries"
+            col = np.empty(pay.size, np.int64)
+            for s in range(W):
+                m = src == s
+                t = tables[s][2 * side]
+                assert (row[m] < t.size).all(), f"rank {r}: side {side} payload past source {s}'s rows"
+                col[m] = t[row[m]]
+            assert (col == key).all(), f"rank {r}: side {side} payload of a row with another key"
+            ids.append((src << 36) | row)
+        order = np.lexsort((ids[1], ids[0]))
+        a, b = ids[0][order], ids[1][order]
+        assert not ((a[1:] == a[:-1]) & (b[1:] == b[:-1])).any(), f"rank {r}: a pair written twice"
+
+
 def case_repeated():
     """Calls with changing sizes and odf on one group: inbox banks, sequence numbers and the verdict
     slots are reused call after call."""
@@ -602,6 +666,7 @@ CASES = {
 }
 if W == 2:
     CASES["plan-clamped"] = case_plan_clamped
+    CASES["count-past-2^31"] = case_count_past_2_31
 
 
 def main():

@@ -6,6 +6,8 @@ import os
 import numpy as np
 import pytest
 
+import keys as K
+
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
@@ -54,7 +56,9 @@ def test_hash_partition_matches_oracle(dj, oracle, n, nparts, npay, hid):
     keys = rng.integers(-(1 << 62), 1 << 62, n, dtype=np.int64)
     if hid == IDENTITY:
         keys = -np.abs(keys) - 1
-    pays = [np.arange(n, dtype=np.int64) * (c + 1) + c for c in range(npay)]
+    # payload c of row i: mix64(base_c + i), full-width words in both 32-bit halves
+    bases = [c << 40 for c in range(npay)]
+    pays = [K.mix64(np.arange(n, dtype=np.int64) + b) for b in bases]
     ko, pos, off = dj.hash_partition(_t(keys), [_t(p) for p in pays], nparts, dj.SEED_NVLINK, hid)
     ko, pos, off = _n(ko), [_n(p) for p in pos], _n(off)
     ok, op, ooff = oracle.hash_partition(keys, pays[0], nparts, oracle.SEED_NVLINK, hid)
@@ -65,10 +69,13 @@ def test_hash_partition_matches_oracle(dj, oracle, n, nparts, npay, hid):
         a = np.sort(pos[0][off[p]:off[p + 1]])
         b = np.sort(op[ooff[p]:ooff[p + 1]])
         assert (a == b).all()
-    # rows stay intact: payload c is a function of payload 0, key is keys[payload0]
-    assert (ko == keys[pos[0]]).all() if n else True
+    # rows stay intact: payload 0 decodes to a row, the key is that row's key and payload c is the
+    # function of that row
+    row = K.unmix64(pos[0]) - bases[0]
+    assert ((row >= 0) & (row < n)).all()
+    assert (ko == keys[row]).all()
     for c in range(1, npay):
-        assert (pos[c] == pos[0] * (c + 1) + c).all()
+        assert (pos[c] == K.mix64(row + bases[c])).all()
 
 
 def test_hash_partition_identity_hash_colocation(dj):

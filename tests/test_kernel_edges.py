@@ -10,8 +10,17 @@ against the CPU oracle (oracle.inner_join / oracle.hash_partition).
                  only the full key comparison separates them;
   capacity       truncated outputs, exact counts, no write past the capacity;
   unaligned      input columns that are offset views (skip_of == 1 in the TMA staging windows);
-  streamed host  dj_distributed_inner_join_i64_host with several probe chunks, and its overflow.
+  streamed host  dj_distributed_inner_join_i64_host with several probe chunks, and its overflow;
+  edge words     0, +-1, INT64_MIN/MAX and the words around the 32-bit half boundaries as keys and
+                 payloads, through every join entry, hash_partition and partition_ids;
+  single bucket  partition tiles whose rows all go to one bucket (one key, one partition, two
+                 partitions alternating), joins with every row in the first or last radix bucket;
+  large counts   join counts past 2^31 out of one build job and past 2^32 over many buckets, exact
+                 through every entry, with valid, distinct rows below a small capacity;
+  checksum       dj_multiset_checksum4 itself, past its grid-stride cap and accumulating.
 
+Every payload is a full-width word (K.mix64 of a row id), so a 32-bit half that is sign-extended
+while a row is packed into or unpacked from its int4 form changes the result.
 The keys are built by inverting the join's hashes (tests/keys.py, pinned by tests/test_keys.py).
 Kernel variants chosen by environment variables are covered by re-running this module in a fresh
 process (test_variant_sweep), since the library caches each choice for the life of the process.
@@ -97,7 +106,8 @@ def _n(t):
 
 
 def _ids(n, base=0):
-    return np.arange(base, base + n, dtype=np.int64)
+    """Payloads of rows base .. base+n-1: full-width words (mix64), decoded with K.unmix64."""
+    return K.mix64(np.arange(base, base + n, dtype=np.int64))
 
 
 def _sub_multiset(sub, ref):
@@ -381,8 +391,8 @@ def test_unaligned_input_columns(dj, oracle, n, mask):
     res = dj.distributed_inner_join(None, *cols_in)
     _assert_rows(dj, oracle, res.cols, res.n_out, ref_n, ref)
 
-    # hash_partition: key = bk, payload 0 = row id, payload 1 = a function of it
-    pay1 = bp * 3 + 1
+    # hash_partition: key = bk, payload 0 = mixed row id, payload 1 = a function of it
+    pay1 = K.mix64(bp)
     keys_t = _column(bk, m & 1, poison_b)
     p0 = _column(bp, m & 2, POISON_PAY)
     p1 = _column(pay1, m & 4, POISON_PAY)
@@ -393,9 +403,9 @@ def test_unaligned_input_columns(dj, oracle, n, mask):
         assert (off == ooff).all()
         for p in range(8):
             assert (np.sort(pos[0][off[p]:off[p + 1]]) == np.sort(op[ooff[p]:ooff[p + 1]])).all()
-        assert (ko == bk[pos[0] - (1 << 20)]).all()
+        assert (ko == bk[K.unmix64(pos[0]) - (1 << 20)]).all()
         if len(pays) == 2:
-            assert (pos[1] == pos[0] * 3 + 1).all()
+            assert (pos[1] == K.mix64(pos[0])).all()
 
 
 # --------------------------------------------------------------------------- streamed host entry
@@ -484,6 +494,366 @@ def test_streamed_host_join_overflow(dj, oracle, swap):
     assert _sub_multiset([o[:cap] for o in out], ref)
     for o in out:
         assert (o[cap:] == SENTINEL).all()
+
+
+def _device_join_raw(dj, lk, lp, rk, rp, cap):
+    """One dj_distributed_inner_join_i64(NULL, ...) call into guarded device columns.
+    Returns (rc, count, the four columns with their guard tails on the host)."""
+    import torch
+
+    L = dj.lib()
+    t = [_t(a) for a in (lk, lp, rk, rp)]
+    outs = [torch.full((cap + GUARD,), SENTINEL, dtype=torch.int64, device="cuda") for _ in range(4)]
+    ws = dj.workspace(L.dj_distributed_inner_join_workspace_bytes(len(lk), len(rk), 1, 1))
+    cnt, opts = C.c_int64(0), dj.JoinOptions(1, 0)
+    rc = L.dj_distributed_inner_join_i64(None, t[0].data_ptr(), t[1].data_ptr(), len(lk), t[2].data_ptr(),
+                                         t[3].data_ptr(), len(rk), *[o.data_ptr() for o in outs], cap,
+                                         C.byref(cnt), C.byref(opts), ws.data_ptr(), ws.numel(), dj._stream())
+    torch.cuda.synchronize()
+    return rc, cnt.value, [_n(o) for o in outs]
+
+
+def _host_join_raw(dj, lk, lp, rk, rp, cap):
+    """One streamed dj_distributed_inner_join_i64_host(NULL, ...) call into guarded pinned columns."""
+    import torch
+
+    L = dj.lib()
+    h_in = list(map(_pinned, (lk, lp, rk, rp)))
+    h_out = [torch.full((cap + GUARD,), SENTINEL, dtype=torch.int64).pin_memory() for _ in range(4)]
+    ws = dj.workspace(L.dj_distributed_inner_join_host_workspace_bytes(len(lk), len(rk), cap, 1, 1))
+    cnt, opts = C.c_int64(0), dj.JoinOptions(1, 0)
+    rc = L.dj_distributed_inner_join_i64_host(None, h_in[0].data_ptr(), h_in[1].data_ptr(), len(lk),
+                                              h_in[2].data_ptr(), h_in[3].data_ptr(), len(rk),
+                                              *[o.data_ptr() for o in h_out], cap, C.byref(cnt), C.byref(opts),
+                                              ws.data_ptr(), ws.numel(), dj._stream())
+    torch.cuda.synchronize()
+    return rc, cnt.value, [o.numpy().copy() for o in h_out]
+
+
+# ------------------------------------------------------------------------------------ edge words
+_M64 = (1 << 64) - 1
+EDGE_WORDS = [0, 1, -1, -(1 << 63), (1 << 63) - 1, 0x7FFFFFFF, 0x80000000, 0xFFFFFFFF, 0x7FFFFFFF_80000000,
+              0x80000000_00000000, 0x80000000_80000000, 0xFFFFFFFF_00000000]
+
+
+def _edge_words():
+    """Every EDGE_WORDS entry +-3 (64-bit wrap), as distinct int64 words."""
+    ws = {((w + d) & _M64) for w in EDGE_WORDS for d in range(-3, 4)}
+    return np.array(sorted(ws), dtype=np.uint64).view(np.int64)
+
+
+def _edge_table(rng, n_pad_build, n_pad_probe):
+    """Build and probe tables keyed by the edge words, each word 1-3 times per side (a few on one
+    side only), padded with random full-width misses.  The payloads are the edge words again
+    (shuffled), then mixed row ids."""
+    ew = _edge_words()
+    i64 = np.iinfo(np.int64)
+
+    def misses(n):
+        m = rng.integers(i64.min, i64.max, n + 64, dtype=np.int64, endpoint=True)
+        return m[~np.isin(m, ew)][:n]
+
+    def side(drop, n_pad, base):
+        keep = ew[rng.permutation(ew.size)[drop:]]
+        k = np.concatenate([np.repeat(keep, rng.integers(1, 4, keep.size)), misses(n_pad)])
+        k = rng.permutation(k)
+        p = np.concatenate([rng.permutation(ew), _ids(k.size, base)])[:k.size]
+        return k, p
+
+    bk, bp = side(3, n_pad_build, 0)
+    pk, pp = side(3, n_pad_probe, 1 << 40)
+    return bk, bp, pk, pp
+
+
+def test_extreme_words_join(dj, oracle):
+    """Edge words as keys and payloads through inner_join and distributed_inner_join(None, ...) in
+    both side orders, row for row against the oracle."""
+    rng = np.random.default_rng(0xE0)
+    bk, bp, pk, pp = _edge_table(rng, 2000, 6000)
+    ref_n, ref = oracle.inner_join(bk, bp, pk, pp)
+    assert ref_n > _edge_words().size
+    tb, tbp, tpk, tpp = _t(bk), _t(bp), _t(pk), _t(pp)
+    cols, n = dj.inner_join(tb, tbp, tpk, tpp)
+    _assert_rows(dj, oracle, cols, n, ref_n, ref)
+    res = dj.distributed_inner_join(None, tb, tbp, tpk, tpp)
+    _assert_rows(dj, oracle, res.cols, res.n_out, ref_n, ref)
+    res = dj.distributed_inner_join(None, tpk, tpp, tb, tbp)
+    _assert_rows(dj, oracle, _swap_sides(res.cols), res.n_out, ref_n, ref)
+
+
+@pytest.mark.parametrize("swap", [False, True], ids=["build-left", "build-right"])
+def test_streamed_host_join_extreme_words(dj, oracle, swap):
+    """The edge-word table through the streamed host entry, its probe side padded past 2^20 rows so
+    that the edge rows are spread over at least two probe chunks."""
+    rng = np.random.default_rng(0xE1 + swap)
+    bk, bp, pk, pp = _edge_table(rng, 2000, (1 << 20) + 4000)
+    assert host_chunks(pk.size)[1] >= 2
+    lk, lp, rk, rp = (pk, pp, bk, bp) if swap else (bk, bp, pk, pp)
+    ref_n, ref = oracle.inner_join(lk, lp, rk, rp)
+    rc, n, out = _host_join_raw(dj, lk, lp, rk, rp, ref_n)
+    assert rc == 0, dj.lib().dj_last_error()
+    _assert_rows(dj, oracle, [o[:n] for o in out], n, ref_n, ref)
+    for o in out:
+        assert (o[n:] == SENTINEL).all()
+
+
+def _assert_partitions(oracle, keys, pays, nparts, hid, ko, pos, off):
+    """hash_partition's result against the oracle: offsets bit-identical, every partition equal to
+    the oracle's as a multiset of whole rows (key and every payload column)."""
+    _, oidx, ooff = oracle.hash_partition(keys, np.arange(keys.size, dtype=np.int64), nparts, oracle.SEED_NVLINK, hid)
+    assert (off == ooff).all()
+    part = np.repeat(np.arange(nparts), np.diff(off))
+    got = [ko] + list(pos)
+    ref = [keys[oidx]] + [p[oidx] for p in pays]
+    og, orf = np.lexsort(got[::-1] + [part]), np.lexsort(ref[::-1] + [part])
+    for a, b in zip(got, ref):
+        assert (a[og] == b[orf]).all()
+
+
+@pytest.mark.parametrize("nparts", [8, 100])
+def test_hash_partition_extreme_words(dj, oracle, nparts):
+    """Edge words as keys and payloads through hash_partition with 1, 2 and 3 payload columns:
+    F = 8 ranks warp-aggregated, F = 100 per row."""
+    rng = np.random.default_rng(nparts)
+    keys, p0, _, _ = _edge_table(rng, 5000, 0)
+    pays = [p0, rng.permutation(p0), K.mix64(p0)]
+    for npay in (1, 2, 3):
+        ko, pos, off = dj.hash_partition(_t(keys), [_t(p) for p in pays[:npay]], nparts, dj.SEED_NVLINK)
+        _assert_partitions(oracle, keys, pays[:npay], nparts, dj.HASH_MURMUR3, _n(ko), [_n(p) for p in pos], _n(off))
+
+
+def test_partition_ids_extreme_words(dj, oracle):
+    """partition_ids of the edge words under both hashes (the identity hash keeps the low word only)."""
+    w = _edge_words()
+    for hid in (dj.HASH_MURMUR3, dj.HASH_IDENTITY):
+        for nparts in (8, 100, 1024):
+            got = _n(dj.partition_ids(_t(w), dj.SEED_NVLINK, nparts, hid))
+            want = oracle.partition_ids(w, oracle.SEED_NVLINK, nparts, hid)
+            assert (got == want).all() and (want == oracle.np_partition_ids(w, oracle.SEED_NVLINK, nparts, hid)).all()
+
+
+# ----------------------------------------------------------------------------- single-bucket tiles
+SB_FANOUTS = [2, 32, 33, 1024]
+SB_N = [4096, 4097, 32769]  # one full 4096-row tile, one row past it, past the 32768-row histogram tile
+SB_DISTS = ["same-key", "last-partition", "last-partition-identity", "alternating"]
+
+
+def _keys_by_partition(oracle, nparts, hid, want, n, rng):
+    """{pid: n distinct random full-width keys whose partition id is pid} for every pid in `want`."""
+    i64 = np.iinfo(np.int64)
+    found = {p: np.empty(0, np.int64) for p in want}
+    while min(v.size for v in found.values()) < n:
+        cand = rng.integers(i64.min, i64.max, 1 << 22, dtype=np.int64, endpoint=True)
+        pid = oracle.partition_ids(cand, oracle.SEED_NVLINK, nparts, hid)
+        for p in want:
+            found[p] = np.unique(np.concatenate([found[p], cand[pid == p]]))
+    return {p: rng.permutation(v)[:n] for p, v in found.items()}
+
+
+@pytest.mark.parametrize("nparts", SB_FANOUTS)
+@pytest.mark.parametrize("dist", SB_DISTS)
+def test_hash_partition_single_bucket_tiles(dj, oracle, dist, nparts):
+    """Tiles whose rows all go to one partition (or to two, alternating), with 1-3 payload columns:
+    one run per tile in the copy-out, tile ranks up to 4095, and __match_any_sync over warps of one
+    or two groups.  Offsets bit-identical, partitions equal as multisets of whole rows."""
+    rng = np.random.default_rng([SB_DISTS.index(dist), nparts])
+    hid = dj.HASH_IDENTITY if dist.endswith("identity") else dj.HASH_MURMUR3
+    nmax = max(SB_N)
+    if dist == "same-key":
+        pool = np.full(nmax, K.mix64(np.array([nparts]))[0])
+    elif dist == "alternating":
+        by = _keys_by_partition(oracle, nparts, hid, [0, nparts - 1], nmax, rng)
+        pool = np.empty(nmax, np.int64)
+        pool[0::2], pool[1::2] = by[0][: (nmax + 1) // 2], by[nparts - 1][: nmax // 2]
+    else:
+        pool = _keys_by_partition(oracle, nparts, hid, [nparts - 1], nmax, rng)[nparts - 1]
+    for n in SB_N:
+        keys = pool[:n]
+        pays = [_ids(n, c << 40) for c in range(3)]
+        pid = oracle.partition_ids(keys, oracle.SEED_NVLINK, nparts, hid)
+        if dist == "alternating":
+            assert (pid[0::2] == 0).all() and (pid[1::2] == nparts - 1).all()
+        else:
+            assert (pid == pid[0]).all() and (dist == "same-key" or pid[0] == nparts - 1)
+        for npay in (1, 2, 3):
+            ko, pos, off = dj.hash_partition(_t(keys), [_t(p) for p in pays[:npay]], nparts, dj.SEED_NVLINK, hid)
+            _assert_partitions(oracle, keys, pays[:npay], nparts, hid, _n(ko), [_n(p) for p in pos], _n(off))
+
+
+SINGLE_BUCKET_PLANS = {
+    "1bit": (TARGET, (1, 0)),
+    "10bit": ((TARGET + 1) * 1024 - 1, (10, 0)),  # largest single-level plan
+    "5+6": ((TARGET + 1) * 1024, (5, 6)),  # smallest two-level plan; last = level-1 31, level-2 63
+}
+
+
+@pytest.mark.parametrize("where", ["first", "last"])
+@pytest.mark.parametrize("plan", list(SINGLE_BUCKET_PLANS))
+def test_join_single_radix_bucket(dj, oracle, plan, where):
+    """Every build and probe row in one radix bucket, the first or the last: distinct build keys
+    (one bucket of up to ~900 build jobs), probe rows half hits and half misses of that bucket."""
+    nb, split = SINGLE_BUCKET_PLANS[plan]
+    assert plan_split(nb) == split
+    bits = sum(split)
+    bucket = 0 if where == "first" else (1 << bits) - 1
+    rng = np.random.default_rng([bits, bucket])
+    nhit = min(nb, 2000)
+    ks = K.keys_in_bucket(bits, bucket, nb + nhit, rng)  # distinct: the last nhit miss every build key
+    bk = ks[:nb]
+    pk = rng.permutation(np.concatenate([rng.choice(bk, nhit, replace=False), ks[nb:]]))
+    assert (K.bucket_of(bk, bits) == bucket).all() and (K.bucket_of(pk, bits) == bucket).all()
+    bp, pp = _ids(nb), _ids(pk.size, 1 << 40)
+    ref_n, ref = oracle.inner_join(bk, bp, pk, pp)
+    assert ref_n == nhit
+    cols, n = dj.inner_join(_t(bk), _t(bp), _t(pk), _t(pp))
+    _assert_rows(dj, oracle, cols, n, ref_n, ref)
+
+
+def test_join_single_key_two_build_jobs(dj, oracle):
+    """One key on both sides, build_chunk + 5 build rows (two build jobs of one bucket) x 1000 probe
+    rows, plus misses: every pair once, row for row."""
+    rng = np.random.default_rng(2)
+    key = np.int64(-0x7FFFFFFF_7FFFFFFF)  # 0x80000000_80000001
+    bk = rng.permutation(np.concatenate([np.full(BC + 5, key), rng.integers(0, 1 << 62, 50, dtype=np.int64)]))
+    pk = rng.permutation(np.concatenate([np.full(1000, key), rng.integers(0, 1 << 62, 300, dtype=np.int64)]))
+    assert plan_split(bk.size) == (1, 0)
+    bp, pp = _ids(bk.size), _ids(pk.size, 1 << 40)
+    ref_n, ref = oracle.inner_join(bk, bp, pk, pp)
+    assert ref_n >= (BC + 5) * 1000
+    cols, n = dj.inner_join(_t(bk), _t(bp), _t(pk), _t(pp))
+    _assert_rows(dj, oracle, cols, n, ref_n, ref)
+
+
+# ------------------------------------------------------------------------ counts past 2^31 / 2^32
+COUNT_CAP = 2_000_000  # output rows actually written: a few million, never the count
+
+
+def analytic_count(a, b):
+    """Matches of an inner join of key columns a and b: the sum over keys of count in a x count in
+    b, in Python integers."""
+    ua, ca = np.unique(a, return_counts=True)
+    ub, cb = np.unique(b, return_counts=True)
+    _, ia, ib = np.intersect1d(ua, ub, assume_unique=True, return_indices=True)
+    return sum(int(x) * int(y) for x, y in zip(ca[ia], cb[ib]))
+
+
+def _assert_hot_rows(cols, hot, lk, lbase, rk, rbase):
+    """Output rows of a hot-key join: equal keys, each a hot key; each payload decodes (unmix64 minus
+    its side's base) to a row of that side holding the key; no (left row, right row) pair twice."""
+    k0, p0, k2, p2 = cols
+    assert (k0 == k2).all() and np.isin(k0, hot).all()
+    rl, rr = K.unmix64(p0) - lbase, K.unmix64(p2) - rbase
+    assert ((rl >= 0) & (rl < lk.size)).all() and ((rr >= 0) & (rr < rk.size)).all()
+    assert (lk[rl] == k0).all() and (rk[rr] == k2).all()
+    assert np.unique(rl * rk.size + rr).size == k0.size
+
+
+def one_job_tables(nprobe):
+    """build_chunk rows of one key against `nprobe` rows of it: all matches in one build job."""
+    key = np.int64(-0x7FFFFFFF_7FFFFFFF)
+    assert plan_split(BC) == (1, 0)
+    return np.full(BC, key), _ids(BC), np.full(nprobe, key), _ids(nprobe, 1 << 40)
+
+
+ONE_JOB_NPROBE = -(-(1 << 31) // BC) + 3 * PC + 1
+
+
+def test_join_count_past_2_31_in_one_build_job(dj, oracle):
+    """build_chunk x (2^31 / build_chunk + 3 probe chunks + 1) matches, all out of one build job,
+    through dj_inner_join_i64 at a capacity of 2M rows: the count is exact, the rows written are
+    valid and distinct, nothing lands past the capacity."""
+    import torch
+
+    bk, bp, pk, pp = one_job_tables(ONE_JOB_NPROBE)
+    want = analytic_count(bk, pk)
+    assert want == BC * ONE_JOB_NPROBE > 1 << 31
+    L = dj.lib()
+    t = [_t(a) for a in (bk, bp, pk, pp)]
+    outs = [torch.full((COUNT_CAP + GUARD,), SENTINEL, dtype=torch.int64, device="cuda") for _ in range(4)]
+    cnt = torch.zeros(1, dtype=torch.int64, device="cuda")
+    ws = dj.workspace(L.dj_inner_join_workspace_bytes(bk.size, pk.size))
+    rc = L.dj_inner_join_i64(*[x.data_ptr() for x in t[:2]], bk.size, *[x.data_ptr() for x in t[2:]], pk.size,
+                             *[o.data_ptr() for o in outs], COUNT_CAP, cnt.data_ptr(), ws.data_ptr(), ws.numel(),
+                             dj._stream())
+    assert rc == 0, L.dj_last_error()
+    assert int(cnt.item()) == want
+    out = [_n(o) for o in outs]
+    _assert_hot_rows([o[:COUNT_CAP] for o in out], bk[:1], bk, 0, pk, 1 << 40)
+    for o in out:
+        assert (o[COUNT_CAP:] == SENTINEL).all()
+
+
+MANY_BUCKETS_HOT = 32
+
+
+def many_bucket_tables(total_probe, rng):
+    """MANY_BUCKETS_HOT hot keys, one per radix bucket of the build side's plan, build_chunk build
+    rows each; `total_probe` probe rows shared evenly among them."""
+    k = MANY_BUCKETS_HOT
+    bits = plan_bits(k * BC)
+    hot = np.concatenate([K.keys_in_bucket(bits, b * (1 << bits) // k, 1, rng) for b in range(k)])
+    assert np.unique(K.bucket_of(hot, bits)).size == k
+    bk = rng.permutation(np.repeat(hot, BC))
+    pk = rng.permutation(np.repeat(hot, -(-total_probe // k)))
+    return hot, bk, _ids(bk.size), pk, _ids(pk.size, 1 << 40)
+
+
+MANY_BUCKETS_NPROBE = -(-(1 << 32) // BC) + MANY_BUCKETS_HOT * PC
+
+
+def _count_past_2_32(dj, run, swap):
+    rng = np.random.default_rng(32 + swap)
+    hot, bk, bp, pk, pp = many_bucket_tables(MANY_BUCKETS_NPROBE, rng)
+    assert pk.size > 1 << 20
+    want = analytic_count(bk, pk)
+    assert want > 1 << 32
+    lk, lp, rk, rp = (pk, pp, bk, bp) if swap else (bk, bp, pk, pp)
+    rc, n, out = run(dj, lk, lp, rk, rp, COUNT_CAP)
+    assert rc == dj.ERR_OVERFLOW, dj.lib().dj_last_error()
+    assert n == want
+    lbase, rbase = (1 << 40, 0) if swap else (0, 1 << 40)
+    _assert_hot_rows([o[:COUNT_CAP] for o in out], hot, lk, lbase, rk, rbase)
+    for o in out:
+        assert (o[COUNT_CAP:] == SENTINEL).all()
+
+
+@pytest.mark.parametrize("swap", [False, True], ids=["build-left", "build-right"])
+def test_join_count_past_2_32_over_buckets(dj, swap):
+    """More than 2^32 matches over 32 buckets through dj_distributed_inner_join_i64(NULL, ...):
+    DJ_ERR_OVERFLOW with the exact count, valid distinct rows below the capacity."""
+    _count_past_2_32(dj, _device_join_raw, swap)
+
+
+@pytest.mark.parametrize("swap", [False, True], ids=["build-left", "build-right"])
+def test_streamed_host_join_count_past_2_32(dj, swap):
+    """The same tables through the streamed host entry: the count is summed over >= 2 probe chunks."""
+    assert host_chunks(MANY_BUCKETS_NPROBE)[1] >= 2
+    _count_past_2_32(dj, _host_join_raw, swap)
+
+
+# -------------------------------------------------------------------------------------- checksum
+def test_multiset_checksum4_matches_oracle(dj, oracle):
+    """dj_multiset_checksum4 on random full-width columns: empty, tiny, and one past the grid cap
+    (sm_count * 16 blocks of 256 threads) so the grid-stride loop runs; two calls accumulating into
+    one result equal the oracle over the concatenated rows."""
+    import torch
+
+    cap = torch.cuda.get_device_properties(0).multi_processor_count * 16 * 256
+    rng = np.random.default_rng(4)
+    i64 = np.iinfo(np.int64)
+    for n in (0, 1, 33, cap + 1001):
+        cols = [rng.integers(i64.min, i64.max, n, dtype=np.int64, endpoint=True) for _ in range(4)]
+        assert dj.multiset_checksum4(*map(_t, cols)) == oracle.multiset_checksum4(*cols)
+    t = [_t(c) for c in cols]
+    out = torch.zeros(2, dtype=torch.int64, device="cuda")
+    L = dj.lib()
+    for lo, hi in ((0, 777), (777, n)):
+        assert L.dj_multiset_checksum4(*[c[lo:hi].data_ptr() for c in t], hi - lo, out.data_ptr(), dj._stream()) == 0
+    a, b = out.tolist()
+    assert (a & _M64, b & _M64) == oracle.multiset_checksum4(*cols)
+    # the same rows in another order and split: a multiset checksum
+    perm = rng.permutation(n)
+    assert dj.multiset_checksum4(*[_t(c[perm]) for c in cols]) == oracle.multiset_checksum4(*cols)
 
 
 # ---------------------------------------------------------------------------------- variant sweep

@@ -77,6 +77,35 @@ def test_hash_restatements_match_header(device_hashes):
     assert (K.slot_hash(keys) == sh).all()
 
 
+def test_mix64_is_a_full_width_bijection():
+    """unmix64 inverts mix64 on edge and random words, matches the splitmix64 finalizer written with
+    Python integers, and mix64 of consecutive ids sets bit 31 and bit 63 both ways (the payloads of
+    the GPU cases carry full-width 32-bit halves)."""
+    rng = np.random.default_rng(64)
+    i64 = np.iinfo(np.int64)
+    edges = np.array([0, 1, -1, 2, -2, i64.min, i64.max, i64.min + 1, i64.max - 1, 0x7FFFFFFF, 0x80000000,
+                      0xFFFFFFFF, 1 << 32, 0x7FFFFFFF80000000, -0x7FFFFFFF80000000, -(1 << 32)], dtype=np.int64)
+    words = np.concatenate([edges, rng.integers(i64.min, i64.max, 100_000, dtype=np.int64, endpoint=True)])
+    assert (K.unmix64(K.mix64(words)) == words).all()
+    assert (K.mix64(K.unmix64(words)) == words).all()
+    assert np.unique(K.mix64(words)).size == np.unique(words).size
+
+    def mix_int(x):
+        m = (1 << 64) - 1
+        x &= m
+        x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & m
+        x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & m
+        return x ^ (x >> 31)
+
+    got = K.mix64(words[:2000]).view(np.uint64)
+    assert [int(g) for g in got] == [mix_int(int(w)) for w in words[:2000]]
+    for base in (0, 1 << 20, 1 << 40, 1 << 48, (1 << 48) + (3 << 36)):
+        m = K.mix64(np.arange(base, base + 4096, dtype=np.int64)).view(np.uint64)
+        for bit in (31, 63):
+            b = (m >> np.uint64(bit)) & np.uint64(1)
+            assert 0 < int(b.sum()) < m.size, (base, bit)
+
+
 @pytest.mark.parametrize("bits", [1, 4, 10, 13])
 def test_constructed_keys_hit_their_bucket_and_slot(device_hashes, bits):
     """keys_in_bucket and slot_twins, checked with the header's hashes rather than the restatements."""
