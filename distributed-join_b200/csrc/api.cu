@@ -6,6 +6,7 @@
 #include <vector>
 #include <cstdarg>
 #include <cstdio>
+#include <cstdlib>
 
 #include "dj_device.cuh"
 #include "dj_internal.h"
@@ -101,14 +102,27 @@ RadixPlan plan_for(int64_t nbuild, bool /*any_segmented*/)
   return plan;
 }
 
-// scratch for one side: partition passes' outputs, offsets and pass workspaces
+// DJ_RADIX_EXACT=1: the join's radix levels size their buckets with exact histograms instead of
+// capacities (for A/B comparison and tests)
+static bool radix_exact()
+{
+  static int v = -1;
+  if (v < 0) {
+    const char* e = getenv("DJ_RADIX_EXACT");
+    v             = (e && e[0] == '1') ? 1 : 0;
+  }
+  return v == 1;
+}
+
+// scratch for one side: partition passes' outputs (capacity-padded: bounded_pass_rows), bucket
+// ranges and pass workspaces
 size_t side_ws_bytes(int64_t span_rows, const RadixPlan& plan, int nseg)
 {
-  const int levels = (plan.bits1 > 0) + (plan.bits2 > 0);
   const int F1 = 1 << plan.bits1, F2 = 1 << plan.bits2;
   size_t total = 4096;
-  total += (size_t)levels * align_up((size_t)span_rows * sizeof(Row) + 256, 256);
-  total += align_up(((size_t)plan.nbuckets + 1) * 8, 256) + align_up(((size_t)F1 + 1) * 8, 256);
+  total += align_up((size_t)(bounded_pass_rows(span_rows, 1, F1) + 8) * sizeof(Row), 256);
+  if (plan.bits2) total += align_up((size_t)(bounded_pass_rows(span_rows, F1, F2) + 8) * sizeof(Row), 256);
+  total += 2 * align_up(((size_t)plan.nbuckets + 1) * 8, 256) + 2 * align_up(((size_t)F1 + 1) * 8, 256);
   size_t pw = pass_workspace_bytes(1, F1, nseg);
   if (plan.bits2) pw = std::max(pw, pass_workspace_bytes(F1, F2, nseg));
   return total + pw + 1024;
@@ -120,84 +134,71 @@ static size_t local_join_ws_bytes(int64_t nb, int64_t np)
   return side_ws_bytes(nb, plan, 0) + side_ws_bytes(np, plan, 0) + 8192;
 }
 
-// Radix-partitions one side of a join into plan.nbuckets row-format buckets (1 or 2 passes).
+// Radix-partitions one side of a join into plan.nbuckets row-format buckets (1 or 2 passes).  By
+// default every pass is bounded (run_bounded_pass: no histogram, buckets with gaps); with
+// DJ_RADIX_EXACT=1 every pass is exact and bucket b ends where bucket b+1 begins.
 int prepare_side(const TableInput& in, const RadixPlan& plan, PreparedSide* out, Arena& arena,
                  cudaStream_t stream)
 {
   const int F1 = 1 << plan.bits1, F2 = 1 << plan.bits2;
   DJ_REQUIRE(plan.bits1 > 0, "inner_join: a radix plan needs at least one level");
-  int64_t* off = arena.take<int64_t>((size_t)plan.nbuckets + 1);
+  DJ_REQUIRE(!in.level1_done || (plan.bits2 && in.d_seg_parent && in.rows),
+             "inner_join: fused level 1 needs a two-level plan and row-format pieces");
+  const bool exact = radix_exact();
+  const bool two   = plan.bits2 > 0 && !in.level1_done;  // this side runs both levels
+  auto ranges = [&](size_t n, int64_t** end) {  // bucket begins; ends are the next begins when exact
+    int64_t* b = arena.take<int64_t>(n + 1);
+    *end       = exact ? (b ? b + 1 : nullptr) : arena.take<int64_t>(n);
+    return b;
+  };
+  int64_t *end = nullptr, *end1 = nullptr;
+  int64_t* beg  = ranges((size_t)plan.nbuckets, &end);
+  int64_t* beg1 = two ? ranges((size_t)F1, &end1) : nullptr;
   const size_t pw = std::max(pass_workspace_bytes(1, F1, in.nseg),
                              plan.bits2 ? pass_workspace_bytes(F1, F2, in.nseg) : (size_t)0);
   char* pass_ws = arena.take<char>(pw);
-  if (!off || !pass_ws) {
+  Row* r1 = two ? arena.take<Row>((size_t)bounded_pass_rows(in.nrows, 1, F1) + 8) : nullptr;
+  const int64_t rows_out = plan.bits2 ? bounded_pass_rows(in.nrows, F1, F2) : bounded_pass_rows(in.nrows, 1, F1);
+  Row* r = arena.take<Row>((size_t)rows_out + 8);
+  if (!beg || !end || (two && (!beg1 || !end1 || !r1)) || !pass_ws || !r) {
     set_error("inner_join: workspace too small");
     return DJ_ERR_WORKSPACE;
   }
-  out->d_off = off;
-  auto set_input = [&](PassBuffers& pb) {
-    pb.in_rows = in.rows;
-    pb.in_key  = in.key;
-    pb.in_pay[0] = in.pay;
-    pb.nrows   = in.nrows;
-    if (in.nseg > 0) {
-      pb.d_seg_begin  = in.d_seg_begin;
-      pb.d_seg_end    = in.d_seg_end;
-      pb.d_seg_parent = in.d_seg_parent;
-      pb.nseg         = in.nseg;
-    }
+  // one radix pass of P parents x F children into `dst`; bucket i = [cb[i], ce[i])
+  auto pass = [&](PassBuffers pb, int level, int P, int F, int shift, Row* dst, int64_t* cb, int64_t* ce) {
+    PassDesc d{1, 0, 0, shift, F, P, 1};
+    pb.out_rows    = dst;
+    pb.d_child_off = cb;
+    if (exact) return run_partition_pass(d, pb, pass_ws, pw, stream);
+    pb.d_child_end = ce;
+    return run_bounded_pass(d, pb, level, pass_ws, pw, stream);
   };
-  if (in.level1_done) {
-    // the exchange delivered level-1 buckets as (source, bucket) segments: run level 2 only
-    if (!plan.bits2 || !in.d_seg_parent || !in.rows) {
-      set_error("inner_join: fused level 1 needs a two-level plan and row-format pieces");
-      return DJ_ERR_ARG;
-    }
-    Row* r2 = arena.take<Row>((size_t)in.nrows + 8);
-    if (!r2) {
-      set_error("inner_join: workspace too small");
-      return DJ_ERR_WORKSPACE;
-    }
-    PassDesc d2{1, 0, 0, 32 - plan.bits1 - plan.bits2, F2, F1, 1};
-    PassBuffers pb2{};
-    set_input(pb2);
-    pb2.out_rows = r2;
-    pb2.d_child_off = off;
-    int rc2 = run_partition_pass(d2, pb2, pass_ws, pw, stream);
-    if (rc2) return rc2;
-    out->rows = r2;
-    return DJ_OK;
-  }
-  Row* r1       = arena.take<Row>((size_t)in.nrows + 8);
-  int64_t* off1 = plan.bits2 ? arena.take<int64_t>((size_t)F1 + 1) : off;
-  if (!r1 || !off1) {
-    set_error("inner_join: workspace too small");
-    return DJ_ERR_WORKSPACE;
-  }
-  PassDesc d1{1, 0, 0, 32 - plan.bits1, F1, 1, 1};
   PassBuffers pb{};
-  set_input(pb);
-  pb.d_seg_parent = nullptr;  // a first level has a single parent
-  pb.out_rows     = r1;
-  pb.d_child_off  = off1;
-  int rc = run_partition_pass(d1, pb, pass_ws, pw, stream);
-  if (rc) return rc;
-  out->rows = r1;
-  if (plan.bits2) {
-    Row* r2 = arena.take<Row>((size_t)in.nrows + 8);
-    if (!r2) {
-      set_error("inner_join: workspace too small");
-      return DJ_ERR_WORKSPACE;
-    }
-    PassDesc d2{1, 0, 0, 32 - plan.bits1 - plan.bits2, F2, F1, 1};
-    PassBuffers pb2{};
-    pb2.in_rows = r1; pb2.out_rows = r2;
-    pb2.nrows = in.nrows; pb2.d_parent_off = off1; pb2.d_child_off = off;
-    rc = run_partition_pass(d2, pb2, pass_ws, pw, stream);
-    if (rc) return rc;
-    out->rows = r2;
+  pb.in_rows   = in.rows;
+  pb.in_key    = in.key;
+  pb.in_pay[0] = in.pay;
+  pb.nrows     = in.nrows;
+  if (in.nseg > 0) {
+    pb.d_seg_begin  = in.d_seg_begin;
+    pb.d_seg_end    = in.d_seg_end;
+    pb.d_seg_parent = in.d_seg_parent;
+    pb.nseg         = in.nseg;
   }
-  return DJ_OK;
+  out->rows    = r;
+  out->d_begin = beg;
+  out->d_end   = end;
+  // the exchange delivered level-1 buckets as (source, bucket) segments: run level 2 only
+  if (in.level1_done) return pass(pb, 1, F1, F2, 32 - plan.bits1 - plan.bits2, r, beg, end);
+  pb.d_seg_parent = nullptr;  // a first level has a single parent
+  if (!two) return pass(pb, 0, 1, F1, 32 - plan.bits1, r, beg, end);
+  int rc = pass(pb, 0, 1, F1, 32 - plan.bits1, r1, beg1, end1);
+  if (rc) return rc;
+  PassBuffers pb2{};
+  pb2.in_rows        = r1;
+  pb2.nrows          = bounded_pass_rows(in.nrows, 1, F1);
+  pb2.d_parent_begin = beg1;
+  pb2.d_parent_end   = end1;
+  return pass(pb2, 1, F1, F2, 32 - plan.bits1 - plan.bits2, r, beg, end);
 }
 
 int join_prepared(const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
@@ -205,8 +206,8 @@ int join_prepared(const PreparedSide& build, const PreparedSide& probe, const Ra
                   cudaStream_t stream)
 {
   JoinBuffers jb{};
-  jb.build = build.rows; jb.d_build_off = build.d_off;
-  jb.probe = probe.rows; jb.d_probe_off = probe.d_off;
+  jb.build = build.rows; jb.d_build_begin = build.d_begin; jb.d_build_end = build.d_end;
+  jb.probe = probe.rows; jb.d_probe_begin = probe.d_begin; jb.d_probe_end = probe.d_end;
   jb.nbuckets = plan.nbuckets;
   for (int c = 0; c < 4; c++) jb.out[c] = out[c];
   jb.out_capacity = out_capacity;
@@ -269,6 +270,12 @@ extern "C" int dj_profile_read(double* h_ms4, int64_t* h_launches4)
   return DJ_OK;
 }
 
+extern "C" int dj_testing_radix_repairs(int64_t* h_out2)
+{
+  DJ_REQUIRE(h_out2, "radix_repairs: bad argument");
+  return read_radix_repairs(h_out2);
+}
+
 extern "C" size_t dj_hash_partition_workspace_bytes(int64_t nrows, int nparts)
 {
   (void)nrows;
@@ -296,9 +303,8 @@ extern "C" int dj_hash_partition_i64(const int64_t* d_key, const int64_t* const*
     buf.in_pay[c]  = h_payload_cols[c];
     buf.out_pay[c] = h_out_payload_cols[c];
   }
-  buf.nrows        = nrows;
-  buf.d_parent_off = nullptr;
-  buf.d_child_off  = d_offsets;
+  buf.nrows       = nrows;
+  buf.d_child_off = d_offsets;
   return run_partition_pass(desc, buf, d_workspace, workspace_bytes, (cudaStream_t)stream);
 }
 

@@ -51,9 +51,13 @@ struct PassBuffers {
   const Row* in_rows = nullptr;
   Row* out_rows      = nullptr;
   int64_t nrows;
-  const int64_t* d_parent_off;  // [P+1] absolute row offsets of the parents; nullptr when P == 1
+  // [P] parent p is rows [d_parent_begin[p], d_parent_end[p]) of the input; nullptr when P == 1
+  const int64_t* d_parent_begin = nullptr;
+  const int64_t* d_parent_end   = nullptr;
   int64_t* d_child_off;         // [P*F+1] out: absolute row offsets of the child buckets
-  // Optional explicit input segments (override d_parent_off): segment i is rows
+                                // (bounded passes: [P*F] first row of every child bucket)
+  int64_t* d_child_end = nullptr;  // [P*F] out, bounded passes: one past every child bucket's last row
+  // Optional explicit input segments (override the parent ranges): segment i is rows
   // [d_seg_begin[i], d_seg_end[i]) of the input and feeds output parent d_seg_parent[i]
   // (nullptr: parent 0).  Used for received tables, which are one padded piece per source rank.
   const int64_t* d_seg_begin = nullptr;
@@ -83,6 +87,10 @@ struct PassDev {
   const int* seg_parent;     // [S] output parent bucket the segment's rows belong to
   unsigned long long* counts;  // [P*F+1]
   unsigned long long* cursor;  // [P*F]
+  // Bounded passes: a (tile, bucket) run whose reserved slice would pass cap_end[bucket] is not
+  // copied; overflow[parent] is set instead (nullptr: exact offsets, no check).
+  const unsigned long long* cap_end;
+  int* overflow;
   const int* hist_tiles;       // [S+1] prefix of hist tiles per segment
   const int* scat_tiles;       // [S+1] prefix of scatter tiles per segment
   int S, P, F;
@@ -108,13 +116,28 @@ size_t pass_workspace_bytes(int P, int F, int nseg = 0);
 int run_partition_pass(const PassDesc& desc, const PassBuffers& buf, void* d_ws, size_t ws_bytes,
                        cudaStream_t stream);
 
+// Bounded ("optimistic") radix pass, mode 1 with row output: no histogram.  Every child bucket gets
+// a capacity from its parent's row count and the scatter runs at once; parents in which a child
+// outgrew its capacity are re-scattered with exact offsets by stream-ordered repair kernels that
+// return at once when nothing overflowed.  Child bucket i is rows [d_child_off[i], d_child_end[i]),
+// with gaps between buckets.  `level` (0 or 1) only selects the repair counter.
+int run_bounded_pass(const PassDesc& desc, const PassBuffers& buf, int level, void* d_ws, size_t ws_bytes,
+                     cudaStream_t stream);
+// Upper bound on the output rows of a bounded pass of `nrows` rows split into P parents x F children,
+// whatever the parents' sizes.
+int64_t bounded_pass_rows(int64_t nrows, int P, int F);
+// Parents repaired per level since the previous read; reading clears the counts.
+int read_radix_repairs(int64_t out[2]);
+
 // Local join of radix-partitioned tables: bucket b of the build side is rows
-// [d_build_off[b], d_build_off[b+1]) of (bk, bp), likewise for the probe side.
+// [d_build_begin[b], d_build_end[b]) of `build`, likewise for the probe side.
 struct JoinBuffers {
   const Row* build;
-  const int64_t* d_build_off;
+  const int64_t* d_build_begin;
+  const int64_t* d_build_end;
   const Row* probe;
-  const int64_t* d_probe_off;
+  const int64_t* d_probe_begin;
+  const int64_t* d_probe_end;
   int nbuckets;
   int64_t* out[4];  // build key, build payload, probe key, probe payload
   int64_t out_capacity;
@@ -144,10 +167,11 @@ struct TableInput {
   const int* d_seg_parent = nullptr;  // level-1 bucket of every segment (only with level1_done)
   bool level1_done        = false;    // the sender already split the rows into plan.bits1 buckets
 };
-// The same side radix-partitioned for the join: bucket b = rows [d_off[b], d_off[b+1]).
+// The same side radix-partitioned for the join: bucket b = rows [d_begin[b], d_end[b]).
 struct PreparedSide {
   const Row* rows;
-  const int64_t* d_off;
+  const int64_t* d_begin;
+  const int64_t* d_end;
 };
 RadixPlan plan_for(int64_t nbuild, bool any_segmented);
 size_t side_ws_bytes(int64_t span_rows, const RadixPlan& plan, int nseg);

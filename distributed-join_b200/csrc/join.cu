@@ -53,9 +53,9 @@ constexpr int kDescBuckets = 128;  // bucket descriptors cached per refill
 
 struct JoinDev {
   const Row* build;
-  const int64_t* boff;
+  const int64_t *bbeg, *bend;  // bucket b = rows [bbeg[b], bend[b]) of build
   const Row* probe;
-  const int64_t* poff;
+  const int64_t *pbeg, *pend;
   int nbuckets;
   int64_t* out[4];
   int64_t out_capacity;
@@ -68,8 +68,8 @@ struct __align__(128) JoinSmem {
   Row brow[2][C::kBuildChunk];
   Row prow[C::kProbeStages][C::kProbeChunk];
   int64_t sout[kOutTiles][4][C::kOutRows];
-  int64_t dboff[kDescBuckets + 1];
-  int64_t dpoff[kDescBuckets + 1];
+  int64_t dbb[kDescBuckets], dbe[kDescBuckets];  // cached bucket ranges, build side
+  int64_t dpb[kDescBuckets], dpe[kDescBuckets];  // probe side
   unsigned long long full_build[2], empty_build[2];
   unsigned long long full_probe[C::kProbeStages], empty_probe[C::kProbeStages];
   unsigned long long sbase[kOutTiles];
@@ -87,7 +87,7 @@ __device__ __forceinline__ void consumer_sync()
 template <class S>
 __device__ __forceinline__ int next_valid_bucket(const S& s, int lb, int nd)
 {
-  while (lb < nd && (s.dboff[lb + 1] == s.dboff[lb] || s.dpoff[lb + 1] == s.dpoff[lb])) lb++;
+  while (lb < nd && (s.dbe[lb] == s.dbb[lb] || s.dpe[lb] == s.dpb[lb])) lb++;
   return lb;
 }
 
@@ -135,9 +135,11 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
   for (int base = lo; base < hi; base += kDescBuckets) {
     const int nd = min(kDescBuckets, hi - base);
     __syncthreads();  // everyone is done with the previous descriptors
-    for (int i = tid; i <= nd; i += C::kThreads) {
-      s.dboff[i] = d.boff[base + i];
-      s.dpoff[i] = d.poff[base + i];
+    for (int i = tid; i < nd; i += C::kThreads) {
+      s.dbb[i] = d.bbeg[base + i];
+      s.dbe[i] = d.bend[base + i];
+      s.dpb[i] = d.pbeg[base + i];
+      s.dpe[i] = d.pend[base + i];
     }
     __syncthreads();
 
@@ -145,8 +147,8 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
       // ------------------------------------------------------------ producer (one lane)
       if (lane == 0) {
         for (int lb = next_valid_bucket(s, 0, nd); lb < nd; lb = next_valid_bucket(s, lb + 1, nd)) {
-          const int64_t b1 = s.dboff[lb + 1], p0 = s.dpoff[lb], p1 = s.dpoff[lb + 1];
-          for (int64_t c0 = s.dboff[lb]; c0 < b1; c0 += C::kBuildChunk) {
+          const int64_t b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
+          for (int64_t c0 = s.dbb[lb]; c0 < b1; c0 += C::kBuildChunk) {
             {
               const int bs = u & 1;
               const int n  = (int)min((int64_t)C::kBuildChunk, b1 - c0);
@@ -170,8 +172,8 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
     } else {
       // ------------------------------------------------------------ consumers
       for (int lb = next_valid_bucket(s, 0, nd); lb < nd; lb = next_valid_bucket(s, lb + 1, nd)) {
-        const int64_t b1 = s.dboff[lb + 1], p0 = s.dpoff[lb], p1 = s.dpoff[lb + 1];
-        for (int64_t c0 = s.dboff[lb]; c0 < b1; c0 += C::kBuildChunk) {
+        const int64_t b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
+        for (int64_t c0 = s.dbb[lb]; c0 < b1; c0 += C::kBuildChunk) {
           // ---- build: fingerprint + row index into a 32-bit slot claimed with atomicCAS; the
           //      staged rows themselves are the row store (no copy)
           const int bs = u & 1;
@@ -373,9 +375,11 @@ int run_bucket_join(const JoinBuffers& jb, bool swap_output_sides, cudaStream_t 
 {
   JoinDev d{};
   d.build    = jb.build;
-  d.boff     = jb.d_build_off;
+  d.bbeg     = jb.d_build_begin;
+  d.bend     = jb.d_build_end;
   d.probe    = jb.probe;
-  d.poff     = jb.d_probe_off;
+  d.pbeg     = jb.d_probe_begin;
+  d.pend     = jb.d_probe_end;
   d.nbuckets = jb.nbuckets;
   for (int c = 0; c < 4; c++) d.out[c] = jb.out[swap_output_sides ? (c + 2) % 4 : c];
   d.out_capacity = jb.out_capacity;

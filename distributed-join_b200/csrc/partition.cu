@@ -14,6 +14,15 @@
 // It replaces cudf::hash_partition (reference call sites src/distributed_join.cpp:213-225,
 // src/shuffle_on.cpp:59-60) in mode 0, and is the join's private sub-partitioner in mode 1.
 //
+// The join's radix levels (mode 1, row output) run as BOUNDED passes instead (run_bounded_pass):
+// no histogram.  bucket_bases_kernel gives every child bucket a capacity from its parent's row
+// count (mean + z*sigma + margin: the bucket bits come from a strong mixing hash) and lays the
+// buckets out with gaps; the scatter drops any run that would pass its bucket's capacity and flags
+// the parent.  Its cursor atomics still count every row, so repair_bases_kernel turns a flagged
+// parent's cursors into exact offsets inside the parent's region, and a second scatter re-runs over
+// that parent's input segments only.  The repair kernels are always enqueued and return at once
+// when no parent is flagged: no host synchronisation.
+//
 // Two scatter families:
 //   * SoA -> SoA (scatter_tma_kernel / scatter_kernel): the public cudf::hash_partition
 //     replacement, columns in, columns out.
@@ -23,6 +32,7 @@
 //     ranking of the next tile.  Input is either the caller's SoA columns or rows.
 #include <cub/device/device_scan.cuh>
 
+#include <cmath>
 #include <cstdlib>
 
 #include "dj_device.cuh"
@@ -69,11 +79,13 @@ __device__ __forceinline__ int find_parent(const int* prefix, int P, int t)
 // ---------------------------------------------------------------- plan
 // One CTA: input segments -> tile prefix tables for the two tile sizes.  Segments come either
 // explicitly (begin/end/parent arrays: e.g. the per-source pieces of a received table), from
-// parent offsets (segment i = parent i), or are the single range [0, nrows).
-__global__ void plan_kernel(const int64_t* parent_off_in, const int64_t* seg_begin_in,
-                            const int64_t* seg_end_in, const int* seg_parent_in, int64_t nrows, int S,
-                            int scatter_tile, int64_t* seg_begin, int64_t* seg_end, int* seg_parent,
-                            int* hist_tiles, int* scat_tiles)
+// parent ranges (segment i = parent i), or are the single range [0, nrows).  With `keep`, a
+// segment whose parent p has keep[p] == 0 is emptied (a bounded pass's repair re-plans its own
+// segments in place this way: only overflowed parents keep their rows).
+__global__ void plan_kernel(const int64_t* parent_begin_in, const int64_t* parent_end_in,
+                            const int64_t* seg_begin_in, const int64_t* seg_end_in, const int* seg_parent_in,
+                            int64_t nrows, int S, int scatter_tile, int64_t* seg_begin, int64_t* seg_end,
+                            int* seg_parent, int* hist_tiles, int* scat_tiles, const int* keep)
 {
   __shared__ int warp_sums[33];
   const int tid = threadIdx.x;
@@ -84,14 +96,15 @@ __global__ void plan_kernel(const int64_t* parent_off_in, const int64_t* seg_beg
       lo     = seg_begin_in[tid];
       hi     = seg_end_in[tid];
       parent = seg_parent_in ? seg_parent_in[tid] : 0;
-    } else if (parent_off_in) {
-      lo = parent_off_in[tid];
-      hi = parent_off_in[tid + 1];
+    } else if (parent_begin_in) {
+      lo = parent_begin_in[tid];
+      hi = parent_end_in[tid];
     } else {
       lo     = 0;
       hi     = nrows;
       parent = 0;
     }
+    if (keep && !keep[parent]) hi = lo;
     seg_begin[tid]  = lo;
     seg_end[tid]    = hi;
     seg_parent[tid] = parent;
@@ -654,8 +667,11 @@ __global__ void __launch_bounds__(THREADS, 1) scatter_rows_kernel(PassDev d)
 
     // ---- reserve + scan (thread b owns bucket b)
     const int cnt = tid < F ? cnt_cur[tid] : 0;
-    unsigned long long gres = 0;
-    if (cnt) gres = atomicAdd(&d.cursor[(size_t)td.parent * F + tid], (unsigned long long)cnt);
+    unsigned long long gres = 0, gend = ~0ull;
+    if (cnt) {
+      gres = atomicAdd(&d.cursor[(size_t)td.parent * F + tid], (unsigned long long)cnt);
+      if (d.cap_end) gend = d.cap_end[(size_t)td.parent * F + tid];
+    }
     if (tid < F) s.s_cnt[st ^ 1][tid] = 0;  // the next tile's counters
     int incl = cnt;
 #pragma unroll
@@ -706,12 +722,17 @@ __global__ void __launch_bounds__(THREADS, 1) scatter_rows_kernel(PassDev d)
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic stores -> visible to the TMA engine
     __syncthreads();  // (D) sorted tile complete
 
-    // ---- copy-out: bucket tid's run [excl, excl+cnt) -> out_rows[gres ...)
+    // ---- copy-out: bucket tid's run [excl, excl+cnt) -> out_rows[gres ...); a run that would pass
+    //      the bucket's capacity is dropped and its parent flagged for repair (the cursor still counts it)
     if (cnt) {
-      Row* dst = (d.part_base ? d.part_base[tid >> d.part_shift] : d.out_rows) + gres;
-      asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst),
-                   "r"(smem_u32(&s.srow[excl])), "r"((uint32_t)cnt * 16u)
-                   : "memory");
+      if (gres + (unsigned long long)cnt <= gend) {
+        Row* dst = (d.part_base ? d.part_base[tid >> d.part_shift] : d.out_rows) + gres;
+        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst),
+                     "r"(smem_u32(&s.srow[excl])), "r"((uint32_t)cnt * 16u)
+                     : "memory");
+      } else {
+        d.overflow[td.parent] = 1;
+      }
     }
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
   }
@@ -754,14 +775,14 @@ bool scatter_lean()
 }
 
 template <int MODE, bool IN_ROWS, bool LEAN>
-int launch_scatter_rows_impl(const PassDev& dev, cudaStream_t stream)
+int launch_scatter_rows_impl(const PassDev& dev, cudaStream_t stream, int prof_cat)
 {
   constexpr int THREADS = 1024, RPT = 4;
   const size_t smem = sizeof(ScatterRowsSmem<THREADS, RPT, IN_ROWS>);
   auto kern         = scatter_rows_kernel<MODE, IN_ROWS, THREADS, RPT, LEAN>;
   DJ_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   {
-    ProfScope prof(DJ_PROF_SCATTER, stream);
+    ProfScope prof(prof_cat, stream);
     kern<<<sm_count(), THREADS, smem, stream>>>(dev);
   }
   DJ_LAUNCH_CHECK();
@@ -769,10 +790,10 @@ int launch_scatter_rows_impl(const PassDev& dev, cudaStream_t stream)
 }
 
 template <int MODE, bool IN_ROWS>
-int launch_scatter_rows(const PassDev& dev, cudaStream_t stream)
+int launch_scatter_rows(const PassDev& dev, cudaStream_t stream, int prof_cat = DJ_PROF_SCATTER)
 {
-  return scatter_lean() ? launch_scatter_rows_impl<MODE, IN_ROWS, true>(dev, stream)
-                        : launch_scatter_rows_impl<MODE, IN_ROWS, false>(dev, stream);
+  return scatter_lean() ? launch_scatter_rows_impl<MODE, IN_ROWS, true>(dev, stream, prof_cat)
+                        : launch_scatter_rows_impl<MODE, IN_ROWS, false>(dev, stream, prof_cat);
 }
 
 size_t scatter_smem_bytes(int npay, int F)
@@ -820,6 +841,103 @@ int launch_scatter_npay(const PassDev& dev, int npay, int F, int64_t span, cudaS
   return DJ_ERR_ARG;
 }
 
+// ---------------------------------------------------------------- bounded passes
+// Capacity of each of F child buckets of a parent holding n rows: mean + z * sigma + margin.  The
+// radix bits come from local_hash (a strong mixer), so a child's size is Binomial(n, 1/F):
+// sigma <= sqrt(mean).  z = 8 leaves a Gaussian tail of ~6e-16 per bucket; the constant margin
+// covers the heavier tail of small means and of duplicate keys (DESIGN.md section 2).
+constexpr double kCapZ       = 8.0;
+constexpr int64_t kCapMargin = 32;
+
+__host__ __device__ __forceinline__ int64_t child_capacity(int64_t n, int F)
+{
+  const double mean = (double)n / F;
+  return (int64_t)(mean + kCapZ * sqrt(mean)) + kCapMargin;
+}
+
+// exclusive scan of one int64 per thread over a 1024-thread block
+__device__ __forceinline__ int64_t block_exclusive_scan64(int64_t v, int64_t* warp_sums)
+{
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int64_t incl = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int64_t t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) warp_sums[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    const int64_t w = warp_sums[lane];
+    int64_t wi     = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int64_t t = __shfl_up_sync(0xffffffffu, wi, o);
+      if (lane >= o) wi += t;
+    }
+    warp_sums[lane] = wi - w;
+  }
+  __syncthreads();
+  return warp_sums[warp] + incl - v;
+}
+
+// Grid = P parents x 1024 threads.  Every CTA sums the segments' rows per parent and scans the
+// parents' regions (F * capacity rows each, laid out back to back from row 0), then lays out its
+// own parent: child j starts at region + j * capacity; its cursor starts there, its capacity ends
+// one capacity later.  The parent's overflow flag is cleared.
+__global__ void __launch_bounds__(1024)
+  bucket_bases_kernel(const int64_t* seg_begin, const int64_t* seg_end, const int* seg_parent, int S, int P, int F,
+                      int64_t* begin, unsigned long long* cursor, unsigned long long* cap_end, int* overflow)
+{
+  __shared__ unsigned long long s_rows[kMaxFanout];
+  __shared__ int64_t warp_sums[32];
+  __shared__ int64_t s_start, s_cap;
+  const int tid = threadIdx.x, p = blockIdx.x;
+  if (tid < P) s_rows[tid] = 0;
+  __syncthreads();
+  if (tid < S) atomicAdd(&s_rows[seg_parent[tid]], (unsigned long long)(seg_end[tid] - seg_begin[tid]));
+  __syncthreads();
+  const int64_t cap   = tid < P ? child_capacity((int64_t)s_rows[tid], F) : 0;
+  const int64_t start = block_exclusive_scan64(cap * F, warp_sums);
+  if (tid == p) {
+    s_start     = start;
+    s_cap       = cap;
+    overflow[p] = 0;
+  }
+  __syncthreads();
+  for (int j = tid; j < F; j += 1024) {
+    const size_t b      = (size_t)p * F + j;
+    const int64_t first = s_start + (int64_t)j * s_cap;
+    begin[b]            = first;
+    cursor[b]           = (unsigned long long)first;
+    cap_end[b]          = (unsigned long long)(first + s_cap);
+  }
+}
+
+__device__ unsigned long long g_radix_repairs[2];  // parents repaired per level (read_radix_repairs)
+
+// Grid = P parents x 1024 threads (F <= 1024: one child per thread).  An overflowed parent's
+// children get exact offsets inside its region: the cursors already hold exact counts (cursor -
+// begin), and the region holds F * capacity >= the parent's rows.  Cursors restart at the new
+// offsets, capacities end at the exact sizes.  Parents that did not overflow return at once.
+__global__ void __launch_bounds__(1024) repair_bases_kernel(int F, int level, int64_t* begin, unsigned long long* cursor,
+                                                            unsigned long long* cap_end, const int* overflow)
+{
+  __shared__ int64_t warp_sums[32];
+  const int tid = threadIdx.x, p = blockIdx.x;
+  if (!overflow[p]) return;
+  if (tid == 0) atomicAdd(&g_radix_repairs[level], 1ull);
+  const size_t b      = (size_t)p * F + tid;
+  const int64_t start = begin[(size_t)p * F];
+  const int64_t cnt   = tid < F ? (int64_t)cursor[b] - begin[b] : 0;
+  const int64_t first = start + block_exclusive_scan64(cnt, warp_sums);  // its barriers order the reads above
+  if (tid < F) {
+    begin[b]   = first;
+    cursor[b]  = (unsigned long long)first;
+    cap_end[b] = (unsigned long long)(first + cnt);
+  }
+}
+
 template <int MODE>
 void launch_hist(const PassDev& dev, int grid, size_t smem, cudaStream_t stream)
 {
@@ -831,7 +949,8 @@ void launch_hist(const PassDev& dev, int grid, size_t smem, cudaStream_t stream)
 
 }  // namespace
 
-// workspace: counts[P*F+1] | cursor[P*F] | parent_off[2] | hist_tiles[P+1] | scat_tiles[P+1] | cub temp
+// workspace: counts[P*F+1] | cursor[P*F] | seg_begin, seg_end, seg_parent[S] | hist_tiles[S+1] |
+// scat_tiles[S+1] | overflow[P] | cub temp.  A bounded pass keeps its capacity ends in `counts`.
 static size_t cub_scan_temp_bytes(size_t n)
 {
   size_t bytes = 0;
@@ -849,12 +968,22 @@ size_t pass_workspace_bytes(int P, int F, int nseg)
   total += align_up(nb * 8, 256);
   total += 2 * align_up(S * 8, 256) + align_up(S * 4, 256);
   total += 2 * align_up((S + 1) * 4, 256);
+  total += align_up((size_t)P * 4, 256);
   total += align_up(cub_scan_temp_bytes(nb + 1), 256);
   return total + 1024;
 }
 
-int pass_histogram(const PassDesc& desc, const PassBuffers& buf, void* d_ws, size_t ws_bytes,
-                   cudaStream_t stream, PassState* state)
+namespace {
+
+struct PassWs {
+  unsigned long long *counts, *cursor;
+  int64_t *seg_begin, *seg_end;
+  int *seg_parent, *hist_tiles, *scat_tiles, *overflow;
+  char* cub_temp;
+  size_t cub_bytes;
+};
+
+int check_pass(const PassDesc& desc, const PassBuffers& buf, void* d_ws, size_t ws_bytes, PassWs* w, int* S_out)
 {
   DJ_REQUIRE(desc.F >= 1 && desc.F <= kMaxFanout, "partition: fan-out %d out of range", desc.F);
   DJ_REQUIRE(desc.P >= 1 && desc.P <= kMaxFanout, "partition: parent count %d out of range", desc.P);
@@ -864,32 +993,43 @@ int pass_histogram(const PassDesc& desc, const PassBuffers& buf, void* d_ws, siz
   DJ_REQUIRE(!buf.out_rows || desc.npay == 1, "partition: row output carries exactly one payload column");
   DJ_REQUIRE(!buf.in_rows || buf.out_rows, "partition: row input needs row output");
   const bool explicit_segs = buf.d_seg_begin != nullptr;
-  DJ_REQUIRE(explicit_segs || desc.P == 1 || buf.d_parent_off != nullptr, "partition: parent offsets missing");
+  DJ_REQUIRE(explicit_segs || desc.P == 1 || (buf.d_parent_begin && buf.d_parent_end),
+             "partition: parent ranges missing");
   const int S = explicit_segs ? buf.nseg : desc.P;
   DJ_REQUIRE(S >= 1 && S <= kMaxFanout, "partition: %d input segments (max %d)", S, kMaxFanout);
   const size_t nb = (size_t)desc.P * desc.F;
   DJ_REQUIRE(desc.align_rows == 1 || nb <= 1024, "partition: aligned buckets need P*F <= 1024");
   Arena arena(d_ws, ws_bytes);
-  auto* counts     = arena.take<unsigned long long>(nb + 1);
-  auto* cursor     = arena.take<unsigned long long>(nb);
-  auto* seg_begin  = arena.take<int64_t>(S);
-  auto* seg_end    = arena.take<int64_t>(S);
-  auto* seg_parent = arena.take<int>(S);
-  auto* hist_tiles = arena.take<int>(S + 1);
-  auto* scat_tiles = arena.take<int>(S + 1);
-  size_t cub_bytes = cub_scan_temp_bytes(nb + 1);
-  auto* cub_temp   = arena.take<char>(cub_bytes);
-  if (!counts || !cursor || !seg_begin || !seg_end || !seg_parent || !hist_tiles || !scat_tiles || !cub_temp) {
+  w->counts     = arena.take<unsigned long long>(nb + 1);
+  w->cursor     = arena.take<unsigned long long>(nb);
+  w->seg_begin  = arena.take<int64_t>(S);
+  w->seg_end    = arena.take<int64_t>(S);
+  w->seg_parent = arena.take<int>(S);
+  w->hist_tiles = arena.take<int>(S + 1);
+  w->scat_tiles = arena.take<int>(S + 1);
+  w->overflow   = arena.take<int>(desc.P);
+  w->cub_bytes  = cub_scan_temp_bytes(nb + 1);
+  w->cub_temp   = arena.take<char>(w->cub_bytes);
+  if (!w->counts || !w->cursor || !w->seg_begin || !w->seg_end || !w->seg_parent || !w->hist_tiles ||
+      !w->scat_tiles || !w->overflow || !w->cub_temp) {
     set_error("partition pass: workspace too small (%zu bytes given)", ws_bytes);
     return DJ_ERR_WORKSPACE;
   }
+  *S_out = S;
+  return DJ_OK;
+}
 
-  DJ_CUDA_TRY(cudaMemsetAsync(counts, 0, (nb + 1) * 8, stream));
-  plan_kernel<<<1, 1024, 0, stream>>>(buf.d_parent_off, buf.d_seg_begin, buf.d_seg_end, buf.d_seg_parent,
-                                      buf.nrows, S, kScatterTile, seg_begin, seg_end, seg_parent, hist_tiles,
-                                      scat_tiles);
+int launch_plan(const PassBuffers& buf, int S, const PassWs& w, cudaStream_t stream)
+{
+  plan_kernel<<<1, 1024, 0, stream>>>(buf.d_parent_begin, buf.d_parent_end, buf.d_seg_begin, buf.d_seg_end,
+                                      buf.d_seg_parent, buf.nrows, S, kScatterTile, w.seg_begin, w.seg_end,
+                                      w.seg_parent, w.hist_tiles, w.scat_tiles, nullptr);
   DJ_LAUNCH_CHECK();
+  return DJ_OK;
+}
 
+PassDev make_dev(const PassDesc& desc, const PassBuffers& buf, int S, const PassWs& w)
+{
   PassDev dev{};
   dev.in_key  = buf.in_key;
   dev.out_key = buf.out_key;
@@ -902,13 +1042,13 @@ int pass_histogram(const PassDesc& desc, const PassBuffers& buf, void* d_ws, siz
   dev.part_base  = nullptr;
   dev.part_shift = 0;
   dev.in_total   = buf.nrows;
-  dev.seg_begin  = seg_begin;
-  dev.seg_end    = seg_end;
-  dev.seg_parent = seg_parent;
-  dev.counts     = counts;
-  dev.cursor     = cursor;
-  dev.hist_tiles = hist_tiles;
-  dev.scat_tiles = scat_tiles;
+  dev.seg_begin  = w.seg_begin;
+  dev.seg_end    = w.seg_end;
+  dev.seg_parent = w.seg_parent;
+  dev.counts     = w.counts;
+  dev.cursor     = w.cursor;
+  dev.hist_tiles = w.hist_tiles;
+  dev.scat_tiles = w.scat_tiles;
   dev.S          = S;
   dev.P          = desc.P;
   dev.F          = desc.F;
@@ -918,6 +1058,22 @@ int pass_histogram(const PassDesc& desc, const PassBuffers& buf, void* d_ws, siz
   dev.pow2       = desc.mode == 2 ? (desc.nparts & (desc.nparts - 1)) == 0 : (desc.F & (desc.F - 1)) == 0;
   dev.nparts     = desc.nparts;
   dev.sub_bits   = desc.sub_bits;
+  return dev;
+}
+
+}  // namespace
+
+int pass_histogram(const PassDesc& desc, const PassBuffers& buf, void* d_ws, size_t ws_bytes,
+                   cudaStream_t stream, PassState* state)
+{
+  PassWs w;
+  int S  = 0;
+  int rc = check_pass(desc, buf, d_ws, ws_bytes, &w, &S);
+  if (rc) return rc;
+  const size_t nb = (size_t)desc.P * desc.F;
+  DJ_CUDA_TRY(cudaMemsetAsync(w.counts, 0, (nb + 1) * 8, stream));
+  if ((rc = launch_plan(buf, S, w, stream))) return rc;
+  const PassDev dev = make_dev(desc, buf, S, w);
 
   const int hist_grid = sm_count() * 4;
   const size_t hsmem  = (size_t)desc.F * sizeof(int);
@@ -935,16 +1091,16 @@ int pass_histogram(const PassDesc& desc, const PassBuffers& buf, void* d_ws, siz
   {
     ProfScope prof(DJ_PROF_OTHER, stream);
     if (desc.align_rows > 1) {
-      aligned_offsets_kernel<<<1, 1024, 0, stream>>>(counts, (int)nb, desc.mode == 2 ? 1 << desc.sub_bits : 1,
+      aligned_offsets_kernel<<<1, 1024, 0, stream>>>(w.counts, (int)nb, desc.mode == 2 ? 1 << desc.sub_bits : 1,
                                                      desc.align_rows, buf.d_child_off, buf.d_child_cnt);
       count_launch(1);
     } else {
-      DJ_CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_temp, cub_bytes, counts,
+      DJ_CUDA_TRY(cub::DeviceScan::ExclusiveSum(w.cub_temp, w.cub_bytes, w.counts,
                                                 (unsigned long long*)buf.d_child_off, (int)(nb + 1),
                                                 stream));
       count_launch(2);
     }
-    DJ_CUDA_TRY(cudaMemcpyAsync(cursor, buf.d_child_off, nb * 8, cudaMemcpyDeviceToDevice, stream));
+    DJ_CUDA_TRY(cudaMemcpyAsync(w.cursor, buf.d_child_off, nb * 8, cudaMemcpyDeviceToDevice, stream));
   }
   state->dev  = dev;
   state->mode = desc.mode;
@@ -968,6 +1124,66 @@ int run_partition_pass(const PassDesc& desc, const PassBuffers& buf, void* d_ws,
   int rc = pass_histogram(desc, buf, d_ws, ws_bytes, stream, &st);
   if (rc) return rc;
   return pass_scatter(st, stream);
+}
+
+// Sum over parents of F * child_capacity(n_p, F) <= sum of (n_p + z * sqrt(F * n_p) + F * (margin + 1))
+// (the +1 absorbs rounding), and sum of sqrt(n_p) <= sqrt(P * nrows) by concavity.
+int64_t bounded_pass_rows(int64_t nrows, int P, int F)
+{
+  const double nb = (double)P * F;
+  return nrows + (int64_t)std::ceil(kCapZ * std::sqrt(nb * (double)nrows)) + (int64_t)nb * (kCapMargin + 1);
+}
+
+int run_bounded_pass(const PassDesc& desc, const PassBuffers& buf, int level, void* d_ws, size_t ws_bytes,
+                     cudaStream_t stream)
+{
+  DJ_REQUIRE(desc.mode == 1 && buf.out_rows && buf.d_child_off && buf.d_child_end && level >= 0 && level < 2,
+             "partition: bounded passes are row-output radix passes");
+  PassWs w;
+  int S  = 0;
+  int rc = check_pass(desc, buf, d_ws, ws_bytes, &w, &S);
+  if (rc) return rc;
+  if ((rc = launch_plan(buf, S, w, stream))) return rc;
+  auto* cursor  = reinterpret_cast<unsigned long long*>(buf.d_child_end);
+  auto* cap_end = w.counts;
+  {
+    ProfScope prof(DJ_PROF_HIST, stream);
+    bucket_bases_kernel<<<desc.P, 1024, 0, stream>>>(w.seg_begin, w.seg_end, w.seg_parent, S, desc.P, desc.F,
+                                                     buf.d_child_off, cursor, cap_end, w.overflow);
+  }
+  DJ_LAUNCH_CHECK();
+  PassDev dev  = make_dev(desc, buf, S, w);
+  dev.cursor   = cursor;
+  dev.cap_end  = cap_end;
+  dev.overflow = w.overflow;
+  rc = buf.in_rows ? launch_scatter_rows<1, true>(dev, stream) : launch_scatter_rows<1, false>(dev, stream);
+  if (rc) return rc;
+
+  // repair, always enqueued: exact offsets for overflowed parents, their segments re-planned in
+  // place (every other segment emptied), and the scatter again over those segments only
+  {
+    ProfScope prof(DJ_PROF_OTHER, stream);
+    repair_bases_kernel<<<desc.P, 1024, 0, stream>>>(desc.F, level, buf.d_child_off, cursor, cap_end, w.overflow);
+    count_launch(1);
+    plan_kernel<<<1, 1024, 0, stream>>>(nullptr, nullptr, w.seg_begin, w.seg_end, w.seg_parent, buf.nrows, S,
+                                        kScatterTile, w.seg_begin, w.seg_end, w.seg_parent, w.hist_tiles,
+                                        w.scat_tiles, w.overflow);
+  }
+  DJ_LAUNCH_CHECK();
+  return buf.in_rows ? launch_scatter_rows<1, true>(dev, stream, DJ_PROF_OTHER)
+                     : launch_scatter_rows<1, false>(dev, stream, DJ_PROF_OTHER);
+}
+
+int read_radix_repairs(int64_t out[2])
+{
+  unsigned long long v[2] = {0, 0};
+  DJ_CUDA_TRY(cudaDeviceSynchronize());
+  DJ_CUDA_TRY(cudaMemcpyFromSymbol(v, g_radix_repairs, sizeof(v)));
+  const unsigned long long zero[2] = {0, 0};
+  DJ_CUDA_TRY(cudaMemcpyToSymbol(g_radix_repairs, zero, sizeof(zero)));
+  out[0] = (int64_t)v[0];
+  out[1] = (int64_t)v[1];
+  return DJ_OK;
 }
 
 const void* partition_module_kernel() { return (const void*)plan_kernel; }

@@ -71,7 +71,7 @@ ABI_SYMBOLS = [
     "dj_comm_allgather_i64", "dj_comm_barrier", "dj_all_to_all", "dj_comm_group_start",
     "dj_comm_group_end", "dj_comm_send", "dj_comm_recv", "dj_distributed_inner_join_workspace_bytes",
     "dj_distributed_inner_join_i64", "dj_distributed_inner_join_host_workspace_bytes",
-    "dj_distributed_inner_join_i64_host", "dj_comm_create_local_group",
+    "dj_distributed_inner_join_i64_host", "dj_comm_create_local_group", "dj_testing_radix_repairs",
 ]
 
 _lib = None
@@ -125,6 +125,7 @@ def lib() -> C.CDLL:
     L.dj_distributed_inner_join_host_workspace_bytes.argtypes = [i64, i64, i64, C.c_int, C.c_int]
     L.dj_distributed_inner_join_i64_host.argtypes = L.dj_distributed_inner_join_i64.argtypes
     L.dj_comm_create_local_group.argtypes = [C.c_int, C.POINTER(vp)]
+    L.dj_testing_radix_repairs.argtypes = [C.POINTER(i64)]
     _lib = L
     return L
 

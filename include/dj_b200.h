@@ -247,6 +247,13 @@ int dj_distributed_inner_join_i64_host(dj_comm_t* comm,
  */
 int dj_comm_create_local_group(int size, dj_comm_t** comms);
 
+/* Testing: how many parent buckets the join's radix levels repaired since the previous call of
+ * this function (h_out2[0]: level 1, h_out2[1]: level 2), summed over every side and call on the
+ * current device; the counts are cleared.  A level repairs a parent when one of its child buckets
+ * outgrew the capacity it was given (the parent is re-scattered with exact offsets; results do not
+ * change).  Synchronises the current device. */
+int dj_testing_radix_repairs(int64_t* h_out2);
+
 #if defined(DJ_BUILDING) && defined(__GNUC__)
 #pragma GCC visibility pop
 #endif
