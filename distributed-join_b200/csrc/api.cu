@@ -102,6 +102,33 @@ RadixPlan plan_for(int64_t nbuild, bool /*any_segmented*/)
   return plan;
 }
 
+// A semi / anti join builds on the right table, which is often tiny next to the left one (a fact
+// table filtered by a small key set).  The join kernel runs at most one CTA per bucket, so its
+// plan gets at least kFilterMinBits bits (1024 buckets: every SM busy with either CTA shape); a
+// bucket then holds less than one build job, and the probe side is spread over all of them.
+RadixPlan filter_plan(int64_t nright)
+{
+  RadixPlan plan = plan_for(nright, false);
+  if (plan.bits1 + plan.bits2 < kFilterMinBits) {
+    plan.bits1    = kFilterMinBits;
+    plan.bits2    = 0;
+    plan.nbuckets = 1 << kFilterMinBits;
+  }
+  return plan;
+}
+
+// rows of the array prepare_side lays a side of `span_rows` rows out into (bucket gaps included)
+static int64_t prepared_rows(int64_t span_rows, const RadixPlan& plan)
+{
+  const int F1 = 1 << plan.bits1, F2 = 1 << plan.bits2;
+  return (plan.bits2 ? bounded_pass_rows(span_rows, F1, F2) : bounded_pass_rows(span_rows, 1, F1)) + 8;
+}
+
+size_t filter_bits_bytes(int64_t span_rows, const RadixPlan& plan)
+{
+  return align_up((size_t)((prepared_rows(span_rows, plan) + 31) / 32) * 4, 256) + 256;
+}
+
 // DJ_RADIX_EXACT=1: the join's radix levels size their buckets with exact histograms instead of
 // capacities (for A/B comparison and tests)
 static bool radix_exact()
@@ -134,6 +161,12 @@ static size_t local_join_ws_bytes(int64_t nb, int64_t np)
   return side_ws_bytes(nb, plan, 0) + side_ws_bytes(np, plan, 0) + 8192;
 }
 
+size_t local_filter_join_workspace(int64_t nl, int64_t nr)
+{
+  const RadixPlan plan = filter_plan(nr);
+  return side_ws_bytes(nr, plan, 0) + side_ws_bytes(nl, plan, 0) + filter_bits_bytes(nl, plan) + 8192;
+}
+
 // Radix-partitions one side of a join into plan.nbuckets row-format buckets (1 or 2 passes).  By
 // default every pass is bounded (run_bounded_pass: no histogram, buckets with gaps); with
 // DJ_RADIX_EXACT=1 every pass is exact and bucket b ends where bucket b+1 begins.
@@ -158,8 +191,8 @@ int prepare_side(const TableInput& in, const RadixPlan& plan, PreparedSide* out,
                              plan.bits2 ? pass_workspace_bytes(F1, F2, in.nseg) : (size_t)0);
   char* pass_ws = arena.take<char>(pw);
   Row* r1 = two ? arena.take<Row>((size_t)bounded_pass_rows(in.nrows, 1, F1) + 8) : nullptr;
-  const int64_t rows_out = plan.bits2 ? bounded_pass_rows(in.nrows, F1, F2) : bounded_pass_rows(in.nrows, 1, F1);
-  Row* r = arena.take<Row>((size_t)rows_out + 8);
+  const int64_t rows_out = prepared_rows(in.nrows, plan);
+  Row* r = arena.take<Row>((size_t)rows_out);
   if (!beg || !end || (two && (!beg1 || !end1 || !r1)) || !pass_ws || !r) {
     set_error("inner_join: workspace too small");
     return DJ_ERR_WORKSPACE;
@@ -184,9 +217,10 @@ int prepare_side(const TableInput& in, const RadixPlan& plan, PreparedSide* out,
     pb.d_seg_parent = in.d_seg_parent;
     pb.nseg         = in.nseg;
   }
-  out->rows    = r;
-  out->d_begin = beg;
-  out->d_end   = end;
+  out->rows     = r;
+  out->d_begin  = beg;
+  out->d_end    = end;
+  out->cap_rows = rows_out;
   // the exchange delivered level-1 buckets as (source, bucket) segments: run level 2 only
   if (in.level1_done) return pass(pb, 1, F1, F2, 32 - plan.bits1 - plan.bits2, r, beg, end);
   pb.d_seg_parent = nullptr;  // a first level has a single parent
@@ -203,7 +237,7 @@ int prepare_side(const TableInput& in, const RadixPlan& plan, PreparedSide* out,
 
 int join_prepared(const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
                   int64_t* const out[4], int64_t out_capacity, int64_t* d_out_count, bool swap,
-                  cudaStream_t stream)
+                  cudaStream_t stream, int kind, uint32_t* d_probe_bits)
 {
   JoinBuffers jb{};
   jb.build = build.rows; jb.d_build_begin = build.d_begin; jb.d_build_end = build.d_end;
@@ -212,7 +246,24 @@ int join_prepared(const PreparedSide& build, const PreparedSide& probe, const Ra
   for (int c = 0; c < 4; c++) jb.out[c] = out[c];
   jb.out_capacity = out_capacity;
   jb.d_out_count  = d_out_count;
+  jb.kind         = kind;
+  jb.d_probe_bits = d_probe_bits;
   return run_bucket_join(jb, swap, stream);
+}
+
+int filter_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
+                         int64_t* out_key, int64_t* out_pay, int64_t out_capacity, int64_t* d_out_count,
+                         Arena& arena, cudaStream_t stream)
+{
+  const size_t words = (size_t)(probe.cap_rows + 31) / 32;
+  uint32_t* bits     = arena.take<uint32_t>(words);
+  if (!bits) {
+    set_error("left_filter_join: workspace too small");
+    return DJ_ERR_WORKSPACE;
+  }
+  DJ_CUDA_TRY(cudaMemsetAsync(bits, 0, words * 4, stream));
+  int64_t* const out[4] = {out_key, out_pay, nullptr, nullptr};
+  return join_prepared(build, probe, plan, out, out_capacity, d_out_count, false, stream, kind, bits);
 }
 
 // Joins (bk,bp)[nb] with (pk,pp)[np]; appends matches at *d_out_count (running, device).
@@ -234,6 +285,21 @@ int local_join(const int64_t* bk, const int64_t* bp, int64_t nb, const int64_t* 
 }
 
 size_t local_join_workspace(int64_t nb, int64_t np) { return local_join_ws_bytes(nb, np); }
+
+int local_filter_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* rk, int64_t nr,
+                      int64_t* out_key, int64_t* out_pay, int64_t out_capacity, int64_t* d_out_count, Arena& arena,
+                      cudaStream_t stream)
+{
+  const RadixPlan plan = filter_plan(nr);
+  // the right table has no payload: its key travels as the payload of its rows
+  TableInput tb{rk, rk, nullptr, nr, nullptr, nullptr, 0}, tp{lk, lp, nullptr, nl, nullptr, nullptr, 0};
+  PreparedSide sb{}, sp{};
+  int rc = prepare_side(tb, plan, &sb, arena, stream);
+  if (rc) return rc;
+  rc = prepare_side(tp, plan, &sp, arena, stream);
+  if (rc) return rc;
+  return filter_join_prepared(kind, sb, sp, plan, out_key, out_pay, out_capacity, d_out_count, arena, stream);
+}
 
 }  // namespace dj
 

@@ -747,8 +747,10 @@ constexpr int kAlignRows = 32;
 
 static inline int64_t pad_rows(int64_t n) { return (n + kAlignRows - 1) / kAlignRows * kAlignRows; }
 
-static size_t dist_ws_bytes(int64_t nl, int64_t nr, int world, int odf, double slack)
+// kind 0: inner join; DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI: semi / anti join (build side = right)
+static size_t dist_ws_bytes(int64_t nl, int64_t nr, int world, int odf, double slack, int kind = 0)
 {
+  if (world <= 1 && kind) return local_filter_join_workspace(nl, nr) + 8192;
   if (world <= 1) return local_join_workspace(nl < nr ? nl : nr, nl < nr ? nr : nl) + 8192;
   const int nparts = world * odf;
   size_t total     = 1 << 16;
@@ -763,8 +765,9 @@ static size_t dist_ws_bytes(int64_t nl, int64_t nr, int world, int odf, double s
            (size_t)odf * 2 * 3 * align_up((size_t)kMaxFanout * 8, 256);
   // join scratch for the largest batch (both sides stay alive until the join kernel has run)
   const int64_t bl = (int64_t)(rl / odf) + 4096, br = (int64_t)(rr / odf) + 4096;
-  const RadixPlan plan = plan_for(bl < br ? bl : br, true);
+  const RadixPlan plan = kind ? filter_plan(br) : plan_for(bl < br ? bl : br, true);
   total += side_ws_bytes(bl, plan, kMaxFanout) + side_ws_bytes(br, plan, kMaxFanout);
+  if (kind) total += filter_bits_bytes(bl, plan);
   return total + 8192;
 }
 
@@ -825,15 +828,15 @@ static double ms_since(std::chrono::high_resolution_clock::time_point t0)
   return std::chrono::duration<double, std::milli>(std::chrono::high_resolution_clock::now() - t0).count();
 }
 
-extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_left_key,
-                                             const int64_t* d_left_payload, int64_t nleft,
-                                             const int64_t* d_right_key,
-                                             const int64_t* d_right_payload, int64_t nright,
-                                             int64_t* d_out_lk, int64_t* d_out_lp,
-                                             int64_t* d_out_rk, int64_t* d_out_rp,
-                                             int64_t out_capacity, int64_t* h_out_count,
-                                             dj_join_options* opts, void* d_workspace,
-                                             size_t workspace_bytes, void* stream)
+// The distributed join of every kind.  kind 0: inner join, out = (left key, left payload, right key,
+// right payload).  DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI: the right table's key column is passed as its
+// payload too (d_right_payload == d_right_key), it is always the build side, and out[0..1] receive
+// the kept left rows (d_out_rk, d_out_rp are unused).
+static int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key, const int64_t* d_left_payload,
+                            int64_t nleft, const int64_t* d_right_key, const int64_t* d_right_payload,
+                            int64_t nright, int64_t* d_out_lk, int64_t* d_out_lp, int64_t* d_out_rk,
+                            int64_t* d_out_rp, int64_t out_capacity, int64_t* h_out_count, dj_join_options* opts,
+                            void* d_workspace, size_t workspace_bytes, void* stream)
 {
   DJ_REQUIRE(nleft >= 0 && nright >= 0 && h_out_count && d_workspace, "distributed_inner_join: bad argument");
   cudaStream_t st   = (cudaStream_t)stream;
@@ -857,16 +860,31 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
 
   if (world == 1) {
     // src/distributed_join.cpp:186-199 -- one rank: the local join is the whole job.
-    const bool swap = build_on_right(nleft, nright);
-    int rc = swap ? local_join(d_right_key, d_right_payload, nright, d_left_key, d_left_payload,
-                               nleft, out, out_capacity, d_count, true, arena, st)
-                  : local_join(d_left_key, d_left_payload, nleft, d_right_key, d_right_payload,
-                               nright, out, out_capacity, d_count, false, arena, st);
+    const bool swap = kind == 0 && build_on_right(nleft, nright);
+    int rc = DJ_OK;
+    if (kind == DJ_JOIN_LEFT_ANTI && nright == 0) {
+      // nothing to match: the anti join keeps every left row
+      const int64_t n = std::min(nleft, out_capacity);
+      if (n > 0) {
+        DJ_CUDA_TRY(cudaMemcpyAsync(d_out_lk, d_left_key, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+        DJ_CUDA_TRY(cudaMemcpyAsync(d_out_lp, d_left_payload, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+      }
+    } else if (kind) {
+      if (nleft > 0 && nright > 0)
+        rc = local_filter_join(kind, d_left_key, d_left_payload, nleft, d_right_key, nright, d_out_lk, d_out_lp,
+                               out_capacity, d_count, arena, st);
+    } else {
+      rc = swap ? local_join(d_right_key, d_right_payload, nright, d_left_key, d_left_payload,
+                             nleft, out, out_capacity, d_count, true, arena, st)
+                : local_join(d_left_key, d_left_payload, nleft, d_right_key, d_right_payload,
+                             nright, out, out_capacity, d_count, false, arena, st);
+    }
     if (rc) return rc;
     DJ_CUDA_TRY(cudaMemcpyAsync(comm ? comm->h_pinned : h_out_count, d_count, 8,
                                 cudaMemcpyDeviceToHost, st));
     DJ_CUDA_TRY(cudaStreamSynchronize(st));
     if (comm) *h_out_count = comm->h_pinned[0];
+    if (kind == DJ_JOIN_LEFT_ANTI && nright == 0) *h_out_count = nleft;
     if (timing) {
       opts->t_join_ms = ms_since(t0);
       // the reference labels this branch's time "Hash partition" (src/distributed_join.cpp:194)
@@ -903,10 +921,11 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
   //         identically), workspace size, and the CUDA IPC identity of the workspace.  Everything a
   //         rank later needs to know about a peer's memory layout follows from these numbers and
   //         from the bucket-count matrix (step 2) by pure arithmetic -- no further agreement rounds.
-  constexpr int kHello = 13;  // nleft, nright, workspace bytes, ipc ok, offset in allocation, handle[8]
+  constexpr int kHello = 14;  // nleft, nright, workspace bytes, ipc ok, offset in allocation, handle[8], kind
   std::vector<int64_t> hello((size_t)world * kHello);
   {
     int64_t mine[kHello] = {nleft, nright, (int64_t)workspace_bytes, 0, 0};
+    mine[13]             = kind;
     if (comm->peer_ok && comm->group) {
       // one address space: the raw workspace pointer stands in for the IPC handle (offset 0)
       mine[3] = 1;
@@ -927,6 +946,12 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
     if (rc) return rc;
   }
   auto H = [&](int r, int f) -> int64_t { return hello[(size_t)r * kHello + f]; };
+  for (int r = 0; r < world; r++)
+    if (H(r, 13) != kind) {  // identical verdict everywhere; nothing is queued but the count reset
+      set_error("distributed join: rank %d asked for join kind %lld, this rank for %d", r, (long long)H(r, 13), kind);
+      cudaStreamSynchronize(st);
+      return DJ_ERR_ARG;
+    }
   int sub_bits = 0;
   RadixPlan plan{0, 0, 1};
   {
@@ -937,8 +962,9 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
       tot[0] += H(r, 0);
       tot[1] += H(r, 1);
     }
-    const int64_t est_build = std::min(tot[0], tot[1]) / nparts + 1;  // rows per rank and batch
-    plan                    = plan_for(est_build, true);
+    // rows per rank and batch; semi / anti always build on the right table
+    const int64_t est_build = (kind ? tot[1] : std::min(tot[0], tot[1])) / nparts + 1;
+    plan                    = kind ? filter_plan(est_build) : plan_for(est_build, true);
     const int bits          = plan.bits1 + plan.bits2;
     int fit                 = 0;  // largest sub_bits with nparts << sub_bits <= kMaxFanout
     while ((nparts << (fit + 1)) <= kMaxFanout) fit++;
@@ -998,7 +1024,8 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
         max_span[t]     = std::max(max_span[t], spans[i]);
       }
     L.join_mark = va.used;
-    L.need      = va.used + side_ws_bytes(max_span[0], plan, nseg) + side_ws_bytes(max_span[1], plan, nseg) + 4096;
+    L.need      = va.used + side_ws_bytes(max_span[0], plan, nseg) + side_ws_bytes(max_span[1], plan, nseg) + 4096 +
+             (kind ? filter_bits_bytes(max_span[0], plan) : 0);
     return L;
   };
   // every rank checks every rank's partition-stage fit: the verdict is identical everywhere
@@ -1376,9 +1403,21 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
           drain_exchange();
           return rc;
         }
+      if (kind == DJ_JOIN_LEFT_ANTI && L.rows > 0) {
+        // no right rows in this batch: the anti join keeps every received left row (a piece has
+        // padding between its sources, so the rows are copied segment by segment)
+        int64_t longest = 0;
+        for (int s = 0; s < G; s++) longest = std::max(longest, L.count[s]);
+        rc = append_segment_rows(L.data, L.d_seg_begin, L.d_seg_end, nseg, longest, d_out_lk, d_out_lp, out_capacity,
+                                 d_count, st);
+        if (rc) {
+          drain_exchange();
+          return rc;
+        }
+      }
       continue;
     }
-    const bool swap = build_on_right(L.rows, R.rows);
+    const bool swap = kind == 0 && build_on_right(L.rows, R.rows);
     PreparedSide side[2];
     for (int t = 0; t < 2; t++) {
       Piece& pc = t ? R : L;
@@ -1398,7 +1437,8 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
       }
       trace.mark(t ? "radix(R) end" : "radix(L) end", st);
     }
-    rc = join_prepared(side[swap ? 1 : 0], side[swap ? 0 : 1], plan, out, out_capacity, d_count, swap, st);
+    rc = kind ? filter_join_prepared(kind, side[1], side[0], plan, d_out_lk, d_out_lp, out_capacity, d_count, arena, st)
+              : join_prepared(side[swap ? 1 : 0], side[swap ? 0 : 1], plan, out, out_capacity, d_count, swap, st);
     if (rc) {
       drain_exchange();
       return rc;
@@ -1494,6 +1534,42 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
     return DJ_ERR_OVERFLOW;
   }
   return DJ_OK;
+}
+
+extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_left_key,
+                                             const int64_t* d_left_payload, int64_t nleft,
+                                             const int64_t* d_right_key,
+                                             const int64_t* d_right_payload, int64_t nright,
+                                             int64_t* d_out_lk, int64_t* d_out_lp,
+                                             int64_t* d_out_rk, int64_t* d_out_rp,
+                                             int64_t out_capacity, int64_t* h_out_count,
+                                             dj_join_options* opts, void* d_workspace,
+                                             size_t workspace_bytes, void* stream)
+{
+  return distributed_join(comm, 0, d_left_key, d_left_payload, nleft, d_right_key, d_right_payload, nright, d_out_lk,
+                          d_out_lp, d_out_rk, d_out_rp, out_capacity, h_out_count, opts, d_workspace, workspace_bytes,
+                          stream);
+}
+
+extern "C" size_t dj_distributed_left_filter_join_workspace_bytes(int64_t nleft, int64_t nright, int world,
+                                                                  int over_decom_factor)
+{
+  return dist_ws_bytes(nleft, nright, world, over_decom_factor < 1 ? 1 : over_decom_factor, 1.15, DJ_JOIN_LEFT_SEMI);
+}
+
+extern "C" int dj_distributed_left_filter_join_i64(dj_comm_t* comm, int kind, const int64_t* d_left_key,
+                                                   const int64_t* d_left_payload, int64_t nleft,
+                                                   const int64_t* d_right_key, int64_t nright, int64_t* d_out_key,
+                                                   int64_t* d_out_payload, int64_t out_capacity,
+                                                   int64_t* h_out_count, dj_join_options* opts, void* d_workspace,
+                                                   size_t workspace_bytes, void* stream)
+{
+  DJ_REQUIRE(kind == DJ_JOIN_LEFT_SEMI || kind == DJ_JOIN_LEFT_ANTI, "left_filter_join: unknown join kind %d", kind);
+  DJ_REQUIRE(out_capacity >= 0 && (out_capacity == 0 || (d_out_key && d_out_payload)),
+             "left_filter_join: bad output columns");
+  return distributed_join(comm, kind, d_left_key, d_left_payload, nleft, d_right_key, d_right_key, nright, d_out_key,
+                          d_out_payload, nullptr, nullptr, out_capacity, h_out_count, opts, d_workspace,
+                          workspace_bytes, stream);
 }
 
 static size_t streamed_ws_bytes(int64_t nleft, int64_t nright, int64_t out_capacity);

@@ -22,6 +22,17 @@
 //                      cudf::concatenate is needed afterwards.
 // Multimap semantics: probing continues past a hit until an empty slot.  Build buckets larger
 // than one chunk (skew / duplicates) are processed chunk by chunk, re-streaming the probe side.
+//
+// Left semi / left anti joins (KIND = DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI) run the same kernel
+// with the right table as the build side and the left table as the probe side.  A probe stops at
+// its first key match and emits the probe row itself, (key, payload), at most once: semi on a
+// match, anti when the cluster ends without one.  When a bucket's build side spans several build
+// jobs, a row's verdict is kept across the jobs in one bit per prepared probe row (d.probe_bits,
+// zeroed before the launch): semi emits a row when its atomicOr finds the bit clear, anti sets
+// bits in every job but the last and emits, in the last, the rows with neither a bit nor a match.
+// The jobs of a bucket run in order in one CTA, and the consumer barrier between two jobs orders
+// the bit updates.  An anti join also runs one (empty) build job for a bucket whose build side is
+// empty, so that its probe rows are all emitted.
 #include <cstdlib>
 
 #include "dj_device.cuh"
@@ -60,7 +71,10 @@ struct JoinDev {
   int64_t* out[4];
   int64_t out_capacity;
   unsigned long long* out_count;
+  uint32_t* probe_bits;  // semi / anti: one bit per row of `probe` (multi-job buckets only)
 };
+
+constexpr int kInner = 0, kSemi = DJ_JOIN_LEFT_SEMI, kAnti = DJ_JOIN_LEFT_ANTI;
 
 template <class C>
 struct __align__(128) JoinSmem {
@@ -83,22 +97,27 @@ __device__ __forceinline__ void consumer_sync()
 }
 
 // Build jobs of the cached descriptor block: (bucket, build chunk) pairs whose bucket is
-// non-empty on both sides.  Every thread walks them identically.
-template <class S>
+// non-empty on both sides (anti: on the probe side).  Every thread walks them identically.
+template <int KIND, class S>
 __device__ __forceinline__ int next_valid_bucket(const S& s, int lb, int nd)
 {
-  while (lb < nd && (s.dbe[lb] == s.dbb[lb] || s.dpe[lb] == s.dpb[lb])) lb++;
+  if constexpr (KIND == kAnti) {
+    while (lb < nd && s.dpe[lb] == s.dpb[lb]) lb++;
+  } else {
+    while (lb < nd && (s.dbe[lb] == s.dbb[lb] || s.dpe[lb] == s.dpb[lb])) lb++;
+  }
   return lb;
 }
 
 // Slot word: bit 31 = occupied, bits 30..11 = 20-bit key fingerprint, bits 10..0 = build row.
 __device__ __forceinline__ uint32_t slot_tag(uint32_t h) { return 0x100000u | (h >> 12); }
 
-template <class C>
+template <class C, int KIND>
 __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
 {
   using Smem = JoinSmem<C>;
   constexpr int kConsumers = C::kConsumers;
+  constexpr int kCols      = KIND == kInner ? 4 : 2;  // output columns
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& s        = *reinterpret_cast<Smem*>(smem_raw);
   const int tid  = threadIdx.x;
@@ -146,15 +165,15 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
     if (is_producer) {
       // ------------------------------------------------------------ producer (one lane)
       if (lane == 0) {
-        for (int lb = next_valid_bucket(s, 0, nd); lb < nd; lb = next_valid_bucket(s, lb + 1, nd)) {
-          const int64_t b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
-          for (int64_t c0 = s.dbb[lb]; c0 < b1; c0 += C::kBuildChunk) {
+        for (int lb = next_valid_bucket<KIND>(s, 0, nd); lb < nd; lb = next_valid_bucket<KIND>(s, lb + 1, nd)) {
+          const int64_t b0 = s.dbb[lb], b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
+          for (int64_t c0 = b0; c0 < b1 || (KIND == kAnti && c0 == b0); c0 += C::kBuildChunk) {
             {
               const int bs = u & 1;
-              const int n  = (int)min((int64_t)C::kBuildChunk, b1 - c0);
+              const int n  = (int)min((int64_t)C::kBuildChunk, b1 - c0);  // anti: 0 for an empty build side
               mbar_wait(&s.empty_build[bs], ((u >> 1) & 1) ^ 1);
               mbar_expect_tx(&s.full_build[bs], (uint32_t)n * 16u);
-              tma_load(s.brow[bs], d.build + c0, (uint32_t)n * 16u, &s.full_build[bs]);
+              if (KIND != kAnti || n > 0) tma_load(s.brow[bs], d.build + c0, (uint32_t)n * 16u, &s.full_build[bs]);
               u++;
             }
             for (int64_t r0 = p0; r0 < p1; r0 += C::kProbeChunk) {
@@ -171,9 +190,12 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
       __syncwarp();  // reconverge before the CTA-wide barrier at the top of the loop
     } else {
       // ------------------------------------------------------------ consumers
-      for (int lb = next_valid_bucket(s, 0, nd); lb < nd; lb = next_valid_bucket(s, lb + 1, nd)) {
-        const int64_t b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
-        for (int64_t c0 = s.dbb[lb]; c0 < b1; c0 += C::kBuildChunk) {
+      for (int lb = next_valid_bucket<KIND>(s, 0, nd); lb < nd; lb = next_valid_bucket<KIND>(s, lb + 1, nd)) {
+        const int64_t b0 = s.dbb[lb], b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
+        // semi / anti: does this bucket's build side span several jobs, and is this its last job
+        const bool multi = KIND != kInner && b1 - b0 > C::kBuildChunk;
+        for (int64_t c0 = b0; c0 < b1 || (KIND == kAnti && c0 == b0); c0 += C::kBuildChunk) {
+          const bool last = c0 + C::kBuildChunk >= b1;
           // ---- build: fingerprint + row index into a 32-bit slot claimed with atomicCAS; the
           //      staged rows themselves are the row store (no copy)
           const int bs = u & 1;
@@ -221,6 +243,63 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
             const uint32_t h    = slot_hash_i64(k);
             const uint32_t want = slot_tag(h);
             uint32_t slot       = h & (C::kSlots - 1);
+            if constexpr (KIND != kInner) {
+              // semi / anti: walk to the first key match or to the end of the cluster
+              bool found = false;
+              if (alive) {
+                while (true) {
+                  const uint32_t e = slots[slot];
+                  if (e == 0u) break;
+                  if ((e >> 11) == want && brow[e & 0x7ffu].key == k) {
+                    found = true;
+                    break;
+                  }
+                  slot = (slot + 1) & (C::kSlots - 1);
+                }
+              }
+              const int64_t prow_at = r0 + tid;  // position of this row in the prepared probe side
+              uint32_t* word        = d.probe_bits + (prow_at >> 5);
+              const uint32_t bit    = 1u << (prow_at & 31);
+              bool emit;
+              if constexpr (KIND == kSemi) {
+                emit = found && (!multi || !(atomicOr(word, bit) & bit));
+              } else {
+                if (multi && found && !last) atomicOr(word, bit);
+                // L2 read: the bits were set by atomics, and L1 may hold the word from an earlier bucket
+                emit = alive && !found && last && (!multi || !(__ldcg(word) & bit));
+              }
+              const unsigned m = __ballot_sync(0xffffffffu, emit);
+              if (m) {
+                const int leader = __ffs(m) - 1;
+                int obase        = 0;
+                if (lane == leader) {
+                  obase = atomicAdd(&s.scnt[cur], __popc(m));
+                  if (obase >= C::kOutRows) atomicSub(&s.scnt[cur], __popc(m));
+                }
+                obase            = __shfl_sync(0xffffffffu, obase, leader);
+                const int pos    = obase + __popc(m & lanemask_lt());
+                const bool spill = emit && pos >= C::kOutRows;
+                if (emit && !spill) {
+                  s.sout[cur][0][pos] = k;
+                  s.sout[cur][1][pos] = v;
+                }
+                const unsigned ms = __ballot_sync(0xffffffffu, spill);
+                if (ms) {
+                  const int sl = __ffs(ms) - 1;
+                  unsigned long long g = 0;
+                  if (lane == sl) g = atomicAdd(d.out_count, (unsigned long long)__popc(ms));
+                  g = __shfl_sync(0xffffffffu, g, sl);
+                  if (spill) {
+                    const int64_t gi = (int64_t)g + __popc(ms & lanemask_lt());
+                    if (gi < d.out_capacity) {
+                      d.out[0][gi] = k;
+                      d.out[1][gi] = v;
+                    }
+                  }
+                }
+              }
+              continue;
+            }
             while (true) {
               bool found = false;
               int idx    = 0;
@@ -292,7 +371,7 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
             // it stays untouched until the job after next, when every thread is past here
             const int64_t gb = (int64_t)s.sbase[pend_tile];
 #pragma unroll
-            for (int c = 0; c < 4; c++)
+            for (int c = 0; c < kCols; c++)
               for (int i = tid; i < pend_n; i += kConsumers)
                 if (gb + i < d.out_capacity) d.out[c][gb + i] = s.sout[pend_tile][c][i];
             if (tid == 0) s.scnt[pend_tile] = 0;
@@ -319,7 +398,7 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
     if (pend_n) {
       const int64_t gb = (int64_t)s.sbase[pend_tile];
 #pragma unroll
-      for (int c = 0; c < 4; c++)
+      for (int c = 0; c < kCols; c++)
         for (int i = tid; i < pend_n; i += kConsumers)
           if (gb + i < d.out_capacity) d.out[c][gb + i] = s.sout[pend_tile][c][i];
     }
@@ -336,11 +415,11 @@ int join_shape()
   return shape;
 }
 
-template <class C>
+template <class C, int KIND>
 int launch_join(const JoinDev& d, int ctas_per_sm, cudaStream_t stream)
 {
   const size_t smem = sizeof(JoinSmem<C>);
-  auto kern         = bucket_join_kernel<C>;
+  auto kern         = bucket_join_kernel<C, KIND>;
   DJ_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = sm_count() * ctas_per_sm;
   if (grid > d.nbuckets) grid = d.nbuckets;
@@ -350,6 +429,40 @@ int launch_join(const JoinDev& d, int ctas_per_sm, cudaStream_t stream)
   }
   DJ_LAUNCH_CHECK();
   return DJ_OK;
+}
+
+template <class C>
+int launch_join_kind(const JoinDev& d, int kind, int ctas_per_sm, cudaStream_t stream)
+{
+  return kind == kSemi   ? launch_join<C, kSemi>(d, ctas_per_sm, stream)
+         : kind == kAnti ? launch_join<C, kAnti>(d, ctas_per_sm, stream)
+                         : launch_join<C, kInner>(d, ctas_per_sm, stream);
+}
+
+// Appends the rows of segments [sb[i], se[i]) of `rows` (blockIdx.y = segment) to a two-column
+// output at the running count: an anti join's probe rows when the build side is empty.
+constexpr int kAppendChunk = 4096;  // rows per output reservation
+
+__global__ void __launch_bounds__(256) append_rows_kernel(const Row* rows, const int64_t* sb, const int64_t* se,
+                                                          int64_t* out_key, int64_t* out_pay, int64_t out_capacity,
+                                                          unsigned long long* out_count)
+{
+  __shared__ unsigned long long base;
+  const int64_t b = sb[blockIdx.y], e = se[blockIdx.y];
+  for (int64_t c0 = b + (int64_t)blockIdx.x * kAppendChunk; c0 < e; c0 += (int64_t)gridDim.x * kAppendChunk) {
+    const int n = (int)min((int64_t)kAppendChunk, e - c0);
+    __syncthreads();  // `base` of the previous chunk has been read
+    if (threadIdx.x == 0) base = atomicAdd(out_count, (unsigned long long)n);
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const int64_t g = (int64_t)base + i;
+      if (g < out_capacity) {
+        const Row r = rows[c0 + i];
+        out_key[g]  = r.key;
+        out_pay[g]  = r.pay;
+      }
+    }
+  }
 }
 
 }  // namespace
@@ -384,9 +497,27 @@ int run_bucket_join(const JoinBuffers& jb, bool swap_output_sides, cudaStream_t 
   for (int c = 0; c < 4; c++) d.out[c] = jb.out[swap_output_sides ? (c + 2) % 4 : c];
   d.out_capacity = jb.out_capacity;
   d.out_count    = (unsigned long long*)jb.d_out_count;
-  return join_shape() == 1 ? launch_join<CfgB>(d, 2, stream) : launch_join<CfgA>(d, 1, stream);
+  d.probe_bits   = jb.d_probe_bits;
+  return join_shape() == 1 ? launch_join_kind<CfgB>(d, jb.kind, 2, stream)
+                           : launch_join_kind<CfgA>(d, jb.kind, 1, stream);
 }
 
-const void* join_module_kernel() { return (const void*)bucket_join_kernel<CfgA>; }
+int append_segment_rows(const Row* rows, const int64_t* d_seg_begin, const int64_t* d_seg_end, int nseg,
+                        int64_t max_seg_rows, int64_t* out_key, int64_t* out_pay, int64_t out_capacity,
+                        int64_t* d_out_count, cudaStream_t stream)
+{
+  if (nseg <= 0 || max_seg_rows <= 0) return DJ_OK;
+  const int64_t chunks = (max_seg_rows + kAppendChunk - 1) / kAppendChunk;
+  const dim3 grid((unsigned)(chunks < 64 ? chunks : 64), (unsigned)nseg);
+  {
+    ProfScope prof(DJ_PROF_OTHER, stream);
+    append_rows_kernel<<<grid, 256, 0, stream>>>(rows, d_seg_begin, d_seg_end, out_key, out_pay, out_capacity,
+                                                 (unsigned long long*)d_out_count);
+  }
+  DJ_LAUNCH_CHECK();
+  return DJ_OK;
+}
+
+const void* join_module_kernel() { return (const void*)bucket_join_kernel<CfgA, kInner>; }
 
 }  // namespace dj

@@ -23,8 +23,12 @@ SEED_IB = 87654321  # src/distributed_join.cpp:160
 DEFAULT_HASH_SEED = 0
 GEN_SEED = 1234  # generate_dataset/generate_dataset.cuh:44
 
+ERR_ARG = 2
 ERR_WORKSPACE = 3
 ERR_OVERFLOW = 5
+
+JOIN_LEFT_SEMI = 1
+JOIN_LEFT_ANTI = 2
 
 
 class DjError(RuntimeError):
@@ -72,6 +76,7 @@ ABI_SYMBOLS = [
     "dj_comm_group_end", "dj_comm_send", "dj_comm_recv", "dj_distributed_inner_join_workspace_bytes",
     "dj_distributed_inner_join_i64", "dj_distributed_inner_join_host_workspace_bytes",
     "dj_distributed_inner_join_i64_host", "dj_comm_create_local_group", "dj_testing_radix_repairs",
+    "dj_distributed_left_filter_join_workspace_bytes", "dj_distributed_left_filter_join_i64",
 ]
 
 _lib = None
@@ -124,6 +129,10 @@ def lib() -> C.CDLL:
     L.dj_distributed_inner_join_host_workspace_bytes.restype = sz
     L.dj_distributed_inner_join_host_workspace_bytes.argtypes = [i64, i64, i64, C.c_int, C.c_int]
     L.dj_distributed_inner_join_i64_host.argtypes = L.dj_distributed_inner_join_i64.argtypes
+    L.dj_distributed_left_filter_join_workspace_bytes.restype = sz
+    L.dj_distributed_left_filter_join_workspace_bytes.argtypes = [i64, i64, C.c_int, C.c_int]
+    L.dj_distributed_left_filter_join_i64.argtypes = [vp, C.c_int, vp, vp, i64, vp, i64, vp, vp, i64, C.POINTER(i64),
+                                                      C.POINTER(JoinOptions), vp, sz, vp]
     L.dj_comm_create_local_group.argtypes = [C.c_int, C.POINTER(vp)]
     L.dj_testing_radix_repairs.argtypes = [C.POINTER(i64)]
     _lib = L
@@ -349,29 +358,18 @@ class JoinResult:
     options: JoinOptions
 
 
-def distributed_inner_join(comm, lk, lp, rk, rp, odf=1, capacity=None, ws=None, outs=None, report_timing=False,
-                           measure_exchange=False):
-    """distributed_inner_join (src/distributed_join.cpp:134-340) on device tensors through the C ABI.
-    Both retry loops are collective: every rank receives DJ_ERR_OVERFLOW / DJ_ERR_WORKSPACE together."""
-    lk, lp, rk, rp = map(_i64dev, (lk, lp, rk, rp))
-    nl, nr = lk.numel(), rk.numel()
+def _collective_join(comm, call, ncols, capacity, ws, ws_bytes, outs, dev):
+    """The retry loops of the distributed joins.  `call(outs, capacity, ws)` runs one join and returns
+    (rc, n_out, options).  Both loops are collective: every rank receives DJ_ERR_OVERFLOW /
+    DJ_ERR_WORKSPACE together, so every rank retries together."""
     world = comm.size if comm else 1
-    dev = lk.device
-    if capacity is None:
-        capacity = max(nl, nr, 1)
     if ws is None:
-        ws = workspace(lib().dj_distributed_inner_join_workspace_bytes(nl, nr, world, odf), dev)
+        ws = workspace(ws_bytes, dev)
     while True:
         if outs is None or outs[0].numel() < capacity:
-            outs = [torch.empty(capacity, dtype=torch.int64, device=dev) for _ in range(4)]
-        cnt = C.c_int64(0)
-        opts = JoinOptions(odf, 1 if report_timing else 0)
-        opts.measure_exchange = 1 if measure_exchange else 0
-        rc = _check(lib().dj_distributed_inner_join_i64(comm.handle if comm else None, _ptr(lk), _ptr(lp), nl,
-                                                        _ptr(rk), _ptr(rp), nr, *[_ptr(o) for o in outs], capacity,
-                                                        C.byref(cnt), C.byref(opts), _ptr(ws), ws.numel(), _stream()),
-                    allow=(ERR_OVERFLOW, ERR_WORKSPACE) if world > 1 else (ERR_OVERFLOW,))
-        n = cnt.value
+            outs = [torch.empty(capacity, dtype=torch.int64, device=dev) for _ in range(ncols)]
+        rc, n, opts = call(outs, capacity, ws)
+        _check(rc, allow=(ERR_OVERFLOW, ERR_WORKSPACE) if world > 1 else (ERR_OVERFLOW,))
         if rc == 0:
             return JoinResult(tuple(o[:n] for o in outs), n, opts)
         if rc == ERR_WORKSPACE:
@@ -385,9 +383,65 @@ def distributed_inner_join(comm, lk, lp, rk, rp, odf=1, capacity=None, ws=None, 
         # every rank must retry together: agree on the largest need
         need = max(comm.allgather_i64([n])) if comm and comm.size > 1 else n
         capacity = need
-        outs = [torch.empty(capacity, dtype=torch.int64, device=dev) for _ in range(4)]
+        outs = [torch.empty(capacity, dtype=torch.int64, device=dev) for _ in range(ncols)]
         if comm and comm.size > 1:
             comm.barrier()
+
+
+def distributed_inner_join(comm, lk, lp, rk, rp, odf=1, capacity=None, ws=None, outs=None, report_timing=False,
+                           measure_exchange=False):
+    """distributed_inner_join (src/distributed_join.cpp:134-340) on device tensors through the C ABI.
+    Both retry loops are collective: every rank receives DJ_ERR_OVERFLOW / DJ_ERR_WORKSPACE together."""
+    lk, lp, rk, rp = map(_i64dev, (lk, lp, rk, rp))
+    nl, nr = lk.numel(), rk.numel()
+    world = comm.size if comm else 1
+    if capacity is None:
+        capacity = max(nl, nr, 1)
+
+    def call(outs, capacity, ws):
+        cnt = C.c_int64(0)
+        opts = JoinOptions(odf, 1 if report_timing else 0)
+        opts.measure_exchange = 1 if measure_exchange else 0
+        rc = lib().dj_distributed_inner_join_i64(comm.handle if comm else None, _ptr(lk), _ptr(lp), nl, _ptr(rk),
+                                                 _ptr(rp), nr, *[_ptr(o) for o in outs], capacity, C.byref(cnt),
+                                                 C.byref(opts), _ptr(ws), ws.numel(), _stream())
+        return rc, cnt.value, opts
+
+    ws_bytes = None if ws is not None else lib().dj_distributed_inner_join_workspace_bytes(nl, nr, world, odf)
+    return _collective_join(comm, call, 4, capacity, ws, ws_bytes, outs, lk.device)
+
+
+def distributed_left_filter_join(comm, kind, lk, lp, rk, odf=1, capacity=None, ws=None, outs=None):
+    """Left semi (kind JOIN_LEFT_SEMI) or left anti (JOIN_LEFT_ANTI) join of (lk, lp) against the keys
+    rk through dj_distributed_left_filter_join_i64.  Returns a JoinResult whose cols are the kept
+    (left key, left payload) rows, trimmed; at N > 1 the rows whose keys this rank owns.  `outs`: two
+    caller-owned columns for the first attempt."""
+    lk, lp, rk = map(_i64dev, (lk, lp, rk))
+    nl, nr = lk.numel(), rk.numel()
+    world = comm.size if comm else 1
+    if capacity is None:
+        capacity = max(nl, 1)
+
+    def call(outs, capacity, ws):
+        cnt = C.c_int64(0)
+        opts = JoinOptions(odf, 0)
+        rc = lib().dj_distributed_left_filter_join_i64(comm.handle if comm else None, kind, _ptr(lk), _ptr(lp), nl,
+                                                       _ptr(rk), nr, _ptr(outs[0]), _ptr(outs[1]), capacity,
+                                                       C.byref(cnt), C.byref(opts), _ptr(ws), ws.numel(), _stream())
+        return rc, cnt.value, opts
+
+    ws_bytes = None if ws is not None else lib().dj_distributed_left_filter_join_workspace_bytes(nl, nr, world, odf)
+    return _collective_join(comm, call, 2, capacity, ws, ws_bytes, outs, lk.device)
+
+
+def distributed_left_semi_join(comm, lk, lp, rk, odf=1, capacity=None, ws=None, outs=None):
+    """Every left row whose key appears in rk, once (EXISTS / IN): see distributed_left_filter_join."""
+    return distributed_left_filter_join(comm, JOIN_LEFT_SEMI, lk, lp, rk, odf, capacity, ws, outs)
+
+
+def distributed_left_anti_join(comm, lk, lp, rk, odf=1, capacity=None, ws=None, outs=None):
+    """Every left row whose key does not appear in rk (NOT EXISTS / NOT IN): see distributed_left_filter_join."""
+    return distributed_left_filter_join(comm, JOIN_LEFT_ANTI, lk, lp, rk, odf, capacity, ws, outs)
 
 
 def distributed_inner_join_host(comm, h_lk, h_lp, h_rk, h_rp, h_outs, odf=1, ws=None):

@@ -231,6 +231,31 @@ int dj_distributed_inner_join_i64_host(dj_comm_t* comm,
                                        void* d_workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * dj_distributed_left_filter_join_i64 -- distributed left semi / left anti join (EXISTS / IN and
+ * NOT EXISTS / NOT IN; cudf::left_semi_join / cudf::left_anti_join) of an int64 key + int64
+ * payload left table against an int64 key column.  kind DJ_JOIN_LEFT_SEMI returns every left row
+ * whose key appears in the right table, DJ_JOIN_LEFT_ANTI every left row whose key does not; each
+ * left row at most once (duplicate right keys never multiply a row), as (left key, left payload)
+ * in unspecified order.  A right table that is empty on every rank gives no rows for semi and all
+ * left rows for anti.  Partition, exchange and the collective protocol are those of
+ * dj_distributed_inner_join_i64: comm NULL or size 1 runs the local join only; at N > 1 rank r
+ * returns the left rows whose keys it owns under the murmur3 rank partition (seed 12345678);
+ * every rank must pass the same kind (otherwise every rank returns DJ_ERR_ARG);
+ * DJ_ERR_WORKSPACE / opts->workspace_needed and the all-rank DJ_ERR_OVERFLOW verdict with an exact
+ * *h_out_count behave as for the inner join.
+ */
+enum { DJ_JOIN_LEFT_SEMI = 1, DJ_JOIN_LEFT_ANTI = 2 };
+size_t dj_distributed_left_filter_join_workspace_bytes(int64_t nleft, int64_t nright, int world,
+                                                       int over_decom_factor);
+int dj_distributed_left_filter_join_i64(dj_comm_t* comm, int kind,
+                                        const int64_t* d_left_key, const int64_t* d_left_payload,
+                                        int64_t nleft, const int64_t* d_right_key, int64_t nright,
+                                        int64_t* d_out_key, int64_t* d_out_payload,
+                                        int64_t out_capacity, int64_t* h_out_count,
+                                        dj_join_options* opts, void* d_workspace,
+                                        size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Testing: an in-process rank group.  Creates `size` communicators (ranks 0..size-1) on the
  * current device in one process; comms[r] is meant to be driven by its own host thread.  The
  * multi-rank join runs unchanged from its first control message to its overflow verdict; only
