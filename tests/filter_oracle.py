@@ -14,7 +14,12 @@ import oracle as O
 def left_semi_join(lk, lp, rk, anti=False):
     """(keys, payloads) of the left rows whose key appears in rk (anti: does not), in left order."""
     lk, lp, rk = (np.ascontiguousarray(a, dtype=np.int64) for a in (lk, lp, rk))
-    keep = np.isin(lk, rk, invert=anti)
+    # membership by binary search in the sorted right keys (np.isin sorts left and right together
+    # with an indirect stable sort: seconds for a right side of millions of keys)
+    srk = np.sort(rk)
+    at = np.minimum(np.searchsorted(srk, lk), max(srk.size - 1, 0))
+    found = srk[at] == lk if srk.size else np.zeros(lk.size, bool)
+    keep = found != anti
     return lk[keep], lp[keep]
 
 

@@ -6,7 +6,9 @@ thread per rank, every rank's result against the CPU oracle for both kinds.
 tests/test_left_filter_join.py runs it in a fresh process per (exchange flavour, W), as
 tests/test_local_group.py runs local_group_worker.py, whose group plumbing (rank threads, streams,
 table helpers) this worker reuses.  Rank r's output must equal the oracle's semi (anti) join of all
-ranks' tables restricted to the left keys r owns (partition id % W == r).
+ranks' tables restricted to the left keys r owns (partition id % W == r).  A case that passes the
+restated overflows to run_and_check also checks the radix repair counts, as local_group_worker.py
+does.
 """
 import ctypes as C
 import os
@@ -26,6 +28,7 @@ import djb200 as dj  # noqa: E402
 import filter_oracle as FO  # noqa: E402
 import local_group_worker as LG  # noqa: E402  (reads W from argv like this worker)
 import oracle as O  # noqa: E402
+import test_radix_repair as RR  # noqa: E402
 from local_group_worker import RankError, W, owner, run_ranks, split, upload  # noqa: E402
 
 KINDS = (("semi", dj.JOIN_LEFT_SEMI), ("anti", dj.JOIN_LEFT_ANTI))
@@ -97,13 +100,29 @@ def join_ranks(dev, kind, odf=1):
     return run_ranks(fn)
 
 
-def run_and_check(tables, odf=1):
-    """Both kinds; per rank, semi and anti together are the left rows it owns."""
+def assert_repairs(tables, exp, over, what):
+    """dj_testing_radix_repairs after one binding call per rank, against the restatement's children
+    over capacity `over` (receiver_overflows)."""
+    calls = 2 if any(e[0].size > max(t[0].size, 1) for e, t in zip(exp, tables)) else 1
+    got, want = LG.radix_repairs(), RR.expected_repairs(over, calls)
+    assert got == want, f"radix repairs{what}: {got}, expected {want} from {over}"
+
+
+def overflows(tables, odf):
+    """The receivers' children over capacity under the filter join's plan, restated."""
+    return RR.receiver_overflows([t[0] for t in tables], [t[2] for t in tables], W, odf, LG.NO_FUSE, True)
+
+
+def run_and_check(tables, odf=1, over=None):
+    """Both kinds; per rank, semi and anti together are the left rows it owns.  With `over`
+    (overflows(tables, odf)), each kind's radix repair counts too."""
     dev = upload(tables)
     got = {}
     for name, kind in KINDS:
         res = join_ranks(dev, kind, odf)
-        check(tables, odf, name == "anti", res, f", {name}")
+        exp = check(tables, odf, name == "anti", res, f", {name}")
+        if over is not None:
+            assert_repairs(tables, exp, over, f", {name}")
         got[name] = res
     own = owner(np.concatenate([t[0] for t in tables]), odf)
     for r in range(W):
@@ -153,6 +172,28 @@ def case_hot_key():
     lk = rng.permutation(np.concatenate([np.full(5000, hot), rng.integers(0, 1 << 40, 60_000 * W, dtype=np.int64)]))
     rk = rng.permutation(np.concatenate([np.full(3000, hot), rng.integers(0, 1 << 40, 40_000 * W, dtype=np.int64)]))
     run_and_check(with_payloads(np.array_split(lk, W), np.array_split(rk, W)))
+
+
+def case_repair_level2_receiver():
+    """A two-level plan from the right side's size; one level-2 child of the left rows rank W-1
+    receives passes the capacity computed from its level-1 bucket's exact size, with rows from every
+    source.  Level 1 fused, the repair re-scatters a parent of W segments; under DJ_NO_FUSE=1 the
+    receiver's level 1 stays clean.  (0, 1) for each kind; the filter bits of the repaired left
+    side are indexed by its repaired layout."""
+    rng = np.random.default_rng([W, 44])
+    totr, totl = LG.two_level_tot(), 100_000 * W
+    b1, b2, sub = RR.dist_radix_plan(totl, totr, W, 1, LG.NO_FUSE, True)
+    assert b2 > 0 and sub == (0 if LG.NO_FUSE else b1), (b1, b2, sub)
+    j, c = 5, 40
+    crowd = LG.crowd_keys(int(2.5 * RR._margin(totl / W / (1 << (b1 + b2)))) + W, W - 1, b1 + b2, (j << b2) | c, rng)
+    rf = rng.integers(-(1 << 62), 1 << 62, totr - crowd.size // 4, dtype=np.int64)
+    rk = rng.permutation(np.concatenate([rf, crowd[:crowd.size // 4]]))
+    lf = np.concatenate([rng.choice(rf, totl // 3), rng.integers(-(1 << 62), 1 << 62, totl - totl // 3, dtype=np.int64)])
+    ls = [rng.permutation(np.concatenate([a, b])) for a, b in zip(np.array_split(lf, W), np.array_split(crowd, W))]
+    tables = with_payloads(ls, split(rk, rng))
+    over = overflows(tables, 1)
+    assert over == [(W - 1, 0, 0, 1, j, c)], over
+    run_and_check(tables, over=over)
 
 
 def case_overflow():
@@ -261,6 +302,7 @@ CASES = {
     "right-slice-empty": case_right_slice_empty,
     "right-table-empty": case_right_table_empty,
     "hot-key": case_hot_key,
+    "repair-level2-receiver": case_repair_level2_receiver,
     "overflow-one-rank": case_overflow,
     "workspace-regrow": case_workspace_regrow,
     "kind-mismatch": case_kind_mismatch,
@@ -278,6 +320,7 @@ def main():
         t0 = time.time()
         print(f"run  {name}", flush=True)
         try:
+            LG.radix_repairs()  # reset: every case counts its own repairs
             CASES[name]()
             print(f"ok   {name} ({time.time() - t0:.1f} s)", flush=True)
         except RankError as e:

@@ -10,6 +10,11 @@ case and exits non-zero when a case failed.
 Rank r's output must equal the oracle's join of all ranks' tables restricted to the keys r owns
 (partition id % W == r), and opts.bytes_sent must be 16 bytes per row r sends to another rank.
 
+Radix repairs: dj_testing_radix_repairs counts the parents the bounded radix passes repaired, per
+device, so it sums over every rank of the group; the main thread reads it (which synchronises the
+device and resets it) before every case and after run_ranks returns.  The expected counts come from
+test_radix_repair.receiver_overflows, the capacity rule restated on the rows each rank receives.
+
 Streams: every rank queues work on W + 2 streams (its caller stream, the communicator's two, W - 1
 push streams).  A stream parked on a peer's flag blocks its hardware queue, so no two of these
 streams may share one.  The driver hands queues out round-robin in stream-creation order, so the
@@ -35,6 +40,7 @@ import torch  # noqa: E402
 import djb200 as dj  # noqa: E402
 import keys as K  # noqa: E402
 import oracle as O  # noqa: E402
+import test_radix_repair as RR  # noqa: E402
 from test_kernel_edges import (BC, GUARD, PC, SENTINEL, SORTED_COMPARE_MAX, TARGET, analytic_count,  # noqa: E402
                                dist_plan)
 
@@ -169,8 +175,32 @@ def join_ranks(dev, odf=1, capacity=None, **kw):
     return run_ranks(fn)
 
 
-def run_and_check(tables, odf=1, **kw):
-    check(tables, odf, join_ranks(upload(tables), odf, **kw))
+def radix_repairs():
+    """(level-1, level-2) parents repaired since the last read, summed over the group's ranks."""
+    out = (C.c_int64 * 2)()
+    assert dj.lib().dj_testing_radix_repairs(out) == 0
+    return out[0], out[1]
+
+
+def calls_of(tables, exp, capacity=None):
+    """Calls the binding makes: one more when any rank's rows exceed its first capacity."""
+    caps = [capacity or max(t[0].size, t[2].size, 1) for t in tables]
+    return 2 if any(e[0].size > c for e, c in zip(exp, caps)) else 1
+
+
+def overflows(tables, odf):
+    """The receivers' children over capacity, (rank, batch, side, level, parent, child), restated."""
+    return RR.receiver_overflows([t[0] for t in tables], [t[2] for t in tables], W, odf, NO_FUSE)
+
+
+def run_and_check(tables, odf=1, over=None, **kw):
+    """The binding on every rank against the oracle.  With `over` (overflows(tables, odf)), also
+    the radix repair counts that follow from it."""
+    exp = expected(tables, odf)
+    check(tables, odf, join_ranks(upload(tables), odf, **kw), exp)
+    if over is not None:
+        got, want = radix_repairs(), RR.expected_repairs(over, calls_of(tables, exp, kw.get("capacity")))
+        assert got == want, f"radix repairs {got}, expected {want} from {over}"
 
 
 def raw_join(comm, t, odf, cap, ws, outs, host=False):
@@ -195,7 +225,9 @@ def case_generator(nb, np_, sel, unique, odf):
     for r in range(W):
         (lk, lp), (rk, rp) = dj.generate_tables_distributed(g, r, W)
         tables.append(tuple(x.cpu().numpy() for x in (lk, lp, rk, rp)))
-    run_and_check(tables, odf)
+    over = overflows(tables, odf)
+    assert over == [], over
+    run_and_check(tables, odf, over)
 
 
 def case_plan_edge(two_level):
@@ -207,7 +239,10 @@ def case_plan_edge(two_level):
     rng = np.random.default_rng([W, two_level])
     lk = rng.integers(0, 2 * tot, tot, dtype=np.int64)
     rk = rng.integers(0, 4 * tot, tot + 5000, dtype=np.int64)
-    run_and_check(with_payloads(split(lk, rng), split(rk, rng)))
+    tables = with_payloads(split(lk, rng), split(rk, rng))
+    over = overflows(tables, 1)
+    assert over == [], over
+    run_and_check(tables, over=over)
 
 
 def case_plan_clamped():
@@ -301,7 +336,13 @@ def case_segments():
         for s in range(W):
             for k, c in ((tables[s][0], cl(s)), (tables[s][2], cr(s))):
                 assert in_seg(k, d, j).sum() == c
-    run_and_check(tables)
+    over = overflows(tables, 1)
+    # Fused, nothing repairs.  Under DJ_NO_FUSE=1 the receivers run level 1 themselves, and on ranks 0
+    # and W-1 one of the 32 level-1 buckets holds only the few placed rows: each other bucket then
+    # carries 1/31 more rows than the mean its capacity assumes (~7.5 sigma at these sizes), so some
+    # pass it and that rank's level-1 pass repairs.  Level 2 sizes its children exactly.
+    assert (over != [] and all(o[3] == 0 for o in over)) if NO_FUSE else over == [], over
+    run_and_check(tables, over=over)
 
 
 def case_empty(kind):
@@ -326,13 +367,24 @@ def case_empty(kind):
 
 def case_hot_key():
     """One key with 3000 left x 2000 right rows dealt over every source: 6M rows on its owner, beyond
-    the first attempt's capacity, so the collective overflow retry runs too."""
+    the first attempt's capacity, so the collective overflow retry runs too.
+
+    Radix repairs: the plan is single-level (~40K build rows per rank: 5 bits, children of ~1.3K-1.7K
+    rows with capacities ~300 rows above that), and the hot key's 3000 (2000) copies all land in one
+    child on its owner.  So on that rank both sides repair their only level-1 parent, in each of the
+    two calls: (4, 0) from one key, whatever the exchange flavour."""
     rng = np.random.default_rng([W, 7])
     hot = np.int64(0x1234_5678_9ABC)
     lk = np.concatenate([np.full(3000, hot), rng.integers(0, 1 << 40, 50_000 * W, dtype=np.int64)])
     rk = np.concatenate([np.full(2000, hot), rng.integers(0, 1 << 40, 40_000 * W, dtype=np.int64)])
     lk, rk = rng.permutation(lk), rng.permutation(rk)
-    run_and_check(with_payloads(np.array_split(lk, W), np.array_split(rk, W)))
+    tables = with_payloads(np.array_split(lk, W), np.array_split(rk, W))
+    own, hb = int(owner(np.array([hot]), 1)[0]), int(K.bucket_of(np.array([hot]), RR.dist_radix_plan(
+        lk.size, rk.size, W, 1, NO_FUSE)[0])[0])
+    over = overflows(tables, 1)
+    assert over == [(own, 0, side, 0, 0, hb) for side in (0, 1)], over
+    assert calls_of(tables, expected(tables, 1)) == 2
+    run_and_check(tables, over=over)
 
 
 def case_slot_twins():
@@ -353,6 +405,87 @@ def case_slot_twins():
                          rng.integers(1 << 61, 1 << 62, nr - base.size - 150, dtype=np.int64)])
     assert lk.size == nl and rk.size == nr
     run_and_check(with_payloads(split(rng.permutation(lk), rng), split(rng.permutation(rk), rng)))
+
+
+def crowd_keys(n, dest, bits, bucket, rng, odf=1, batch=0):
+    """n distinct keys in radix bucket `bucket` of a `bits`-bit plan that batch `batch` of rank
+    `dest` receives."""
+    nparts = W * odf
+    out = np.empty(0, np.int64)
+    while out.size < n:
+        k = K.keys_in_bucket(bits, bucket, 2 * nparts * (n - out.size) + 64, rng)
+        out = np.concatenate([out, k[O.partition_ids(k, SEED, nparts) == batch * W + dest]])
+    return out[:n]
+
+
+def crowded_tables(tot, crowd, rng):
+    """Left: `tot` spread keys and the `crowd` keys, the crowd dealt evenly over every source, so a
+    receiver gathers the crowded bucket from W segments.  Right: `tot` keys, an eighth of them left
+    keys, with a sixteenth of the crowd among them."""
+    lf = rng.integers(-(1 << 62), 1 << 62, tot, dtype=np.int64)
+    nc = crowd.size // 16
+    rk = np.concatenate([rng.choice(lf, tot // 8 - nc), crowd[:nc],
+                         rng.integers(-(1 << 62), 1 << 62, tot - tot // 8, dtype=np.int64)])
+    ls = [rng.permutation(np.concatenate([a, b])) for a, b in zip(np.array_split(lf, W), np.array_split(crowd, W))]
+    return with_payloads(ls, split(rng.permutation(rk), rng))
+
+
+def two_level_tot():
+    """Rows per table that give a two-level plan (5 + 6 bits under shape A), level 1 fused at W <= 4."""
+    return (TARGET + 1) * 1024 * W * 11 // 10
+
+
+def case_repair_level2_receiver():
+    """One level-2 child on rank W-1 passes the capacity computed from its level-1 bucket's exact
+    size; its rows come from every source.  Level 1 fused: the bucket is a parent of W segments, one
+    per source, spread over W padded source runs, and the repair re-scatters all of them.
+    DJ_NO_FUSE=1: level 1 runs on the receiver and stays inside its capacities.  (0, 1) either way."""
+    rng = np.random.default_rng([W, 41])
+    tot = two_level_tot()
+    b1, b2, sub = RR.dist_radix_plan(tot + 1, tot, W, 1, NO_FUSE)
+    assert b2 > 0 and sub == (0 if NO_FUSE else b1), (b1, b2, sub)
+    j, c = 3, 21  # the crowded level-1 bucket (sub-bucket) is not 0
+    m2 = tot / W / (1 << (b1 + b2))
+    crowd = crowd_keys(int(2.5 * RR._margin(m2)) + W, W - 1, b1 + b2, (j << b2) | c, rng)
+    tables = crowded_tables(tot, crowd, rng)
+    over = overflows(tables, 1)
+    assert over == [(W - 1, 0, 0, 1, j, c)], over
+    run_and_check(tables, over=over)
+
+
+def case_repair_level1_receiver():
+    """One (destination, sub-bucket) crowded beyond its level-1 capacity, its rows spread over the
+    children.  Level 1 fused: the senders' partition counts exactly, nothing repairs (0, 0).
+    DJ_NO_FUSE=1: the receiver's level-1 pass repairs it (1, 0); level 2 then sizes its children
+    from the exact bucket and stays clean."""
+    rng = np.random.default_rng([W, 42])
+    tot = two_level_tot()
+    b1, b2, _ = RR.dist_radix_plan(tot + 1, tot, W, 1, NO_FUSE)
+    j = 17
+    crowd = crowd_keys(int(2 * RR._margin(tot / W / (1 << b1))), W - 1, b1, j, rng)
+    tables = crowded_tables(tot, crowd, rng)
+    lkeys, rkeys = [t[0] for t in tables], [t[2] for t in tables]
+    over = {}
+    for no_fuse, want in ((True, [(W - 1, 0, 0, 0, 0, j)]), (False, [])):
+        over[no_fuse] = RR.receiver_overflows(lkeys, rkeys, W, 1, no_fuse)
+        assert over[no_fuse] == want, (no_fuse, over[no_fuse])
+    run_and_check(tables, over=over[NO_FUSE])
+
+
+def case_repair_odf2():
+    """odf 2, single-level plan: one child of batch 1 on rank W-1 passes its capacity, batch 0 is
+    clean.  The two batches share the join scratch: (1, 0)."""
+    rng = np.random.default_rng([W, 43])
+    odf, est = 2, 200_000
+    tot = est * W * odf
+    b1, b2, _ = RR.dist_radix_plan(tot + 1, tot, W, odf, NO_FUSE)
+    assert b2 == 0, (b1, b2)
+    c = 77 % (1 << b1)
+    crowd = crowd_keys(int(2.5 * RR._margin(est / (1 << b1))) + W, W - 1, b1, c, rng, odf, 1)
+    tables = crowded_tables(tot, crowd, rng)
+    over = overflows(tables, odf)
+    assert over == [(W - 1, 1, 0, 0, 0, c)], over
+    run_and_check(tables, odf, over)
 
 
 def skewed_tables():
@@ -653,6 +786,9 @@ CASES = {
     "empty-rank-slice": lambda: case_empty("rank-slice"),
     "empty-right-table": lambda: case_empty("right-table"),
     "hot-key": case_hot_key,
+    "repair-level2-receiver": case_repair_level2_receiver,
+    "repair-level1-receiver": case_repair_level1_receiver,
+    "repair-odf2": case_repair_odf2,
     "slot-twins": case_slot_twins,
     "workspace-regrow": case_workspace_regrow,
     "overflow": case_overflow,
@@ -681,6 +817,7 @@ def main():
         t0 = time.time()
         print(f"run  {name}", flush=True)
         try:
+            radix_repairs()  # reset: every case counts its own repairs
             CASES[name]()
             print(f"ok   {name} ({time.time() - t0:.1f} s)", flush=True)
         except RankError as e:

@@ -4,8 +4,10 @@ capacity is repaired (re-scattered with exact offsets).  Keys built by inverting
 (tests/keys.py) force each kind of overflow; every result is compared row for row with the oracle,
 and dj_testing_radix_repairs says which level repaired how many parents.
 
-The plan of a 2M-row build side is two levels, 5 + 6 bits (shape A, 1536-row buckets): 32 level-1
-parents of ~62K rows, each split into 64 children of ~1K rows.
+The plan of a 2M-row build side is two levels: 5 + 6 bits under shape A (1536-row buckets, 32
+level-1 parents of ~62K rows, each split into 64 children of ~1K rows), 6 + 6 under shape B.  The
+plans come from the restatement in test_radix_repair.py, so the module runs under either shape;
+under DJ_RADIX_EXACT=1 (exact histograms) every case expects no repair and the same rows.
 """
 import ctypes as C
 import os
@@ -16,16 +18,21 @@ import numpy as np
 import pytest
 
 import keys as K
+from test_radix_repair import expected_repairs, radix_plan, side_overflows, tagged
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NB = 2_000_000
-BITS1, BITS = 5, 11  # plan of NB build rows: level 1 = top 5 bits, level 2 = the next 6
+BITS1, BITS2 = radix_plan(NB)  # level 1 = the top BITS1 bits of the local hash, level 2 = the next BITS2
+BITS = BITS1 + BITS2
 HOT1 = 19  # the level-1 bucket the adversarial tables crowd
 
 
-def _shape_a():
-    if os.environ.get("DJ_JOIN_SHAPE", "")[:1] in ("B", "b") or os.environ.get("DJ_RADIX_EXACT") == "1":
-        pytest.skip("the plans and repair counts below are those of the default bounded passes, shape A")
+def _want(bk, pk, literal):
+    """The repairs of one join of bk with pk: derived from the capacity restatement, which must
+    agree with the count the case was built for."""
+    over = tagged(("build",), side_overflows(bk, BITS1, BITS2)) + tagged(("probe",), side_overflows(pk, BITS1, BITS2))
+    assert expected_repairs(over) == ((0, 0) if os.environ.get("DJ_RADIX_EXACT") == "1" else literal), over
+    return expected_repairs(over)
 
 
 def _repairs(dj):
@@ -86,21 +93,23 @@ def _join(dj, bk, pk, ws=None):
 def test_level1_overflow(dj, oracle, side):
     """Most rows of one side in one level-1 bucket: that side's level 1 re-scatters its whole table,
     its level 2 then splits the crowded parent from its exact count."""
-    _shape_a()
     rng = np.random.default_rng({"build": 1, "probe": 2, "both": 3}[side])
     bk = _crowded(NB, rng) if side != "probe" else rng.integers(-(1 << 62), 1 << 62, NB)
     bk = np.unique(bk)
     assert (K.bucket_of(bk, BITS1) == HOT1).mean() > (0.6 if side != "probe" else 0.0)
     pk = _probe_for(bk, NB + NB // 4, rng, crowd=side != "build")
+    want = _want(bk, pk, ({"build": 1, "probe": 1, "both": 2}[side], 0))
     _repairs(dj)
     cols, n, bp, pp = _join(dj, bk, pk)
-    assert _repairs(dj) == ({"build": 1, "probe": 1, "both": 2}[side], 0)
+    assert _repairs(dj) == want
     _check(dj, oracle, cols, n, bk, bp, pk, pp)
 
 
-def _one_child_overfull(rng, per=900, extra=700, hot=(7 << 6) | 45):
-    """`per` distinct keys in every level-2 bucket of the 11-bit plan and `extra` more in bucket `hot`:
-    its parent stays inside its level-1 capacity, the child outgrows its level-2 capacity."""
+def _one_child_overfull(rng, extra=700, hot=(7 << BITS2) | 45):
+    """92 % of a full bucket's distinct keys in every level-2 bucket of the plan and `extra` more in
+    bucket `hot`: its parent stays inside its level-1 capacity, the child outgrows its level-2
+    capacity."""
+    per = int(0.92 * (NB >> BITS))
     counts = np.full(1 << BITS, per)
     counts[hot] += extra
     return rng.permutation(np.concatenate([K.keys_in_bucket(BITS, b, int(c), rng) for b, c in enumerate(counts)]))
@@ -108,14 +117,15 @@ def _one_child_overfull(rng, per=900, extra=700, hot=(7 << 6) | 45):
 
 @pytest.mark.gpu
 def test_level2_overflow_in_one_parent(dj, oracle):
-    _shape_a()
     rng = np.random.default_rng(4)
-    hot = (7 << 6) | 45
-    bk = _one_child_overfull(rng, hot=hot)  # 1,843,900 rows: the same 5 + 6 bit plan
+    hot = (7 << BITS2) | 45
+    bk = _one_child_overfull(rng, hot=hot)
+    assert radix_plan(bk.size) == (BITS1, BITS2)  # the same plan as NB rows
     pk = _probe_for(bk, bk.size, rng, False, BITS, hot)
+    want = _want(bk, pk, (0, 1))
     _repairs(dj)
     cols, n, bp, pp = _join(dj, bk, pk)
-    assert _repairs(dj) == (0, 1)
+    assert _repairs(dj) == want
     _check(dj, oracle, cols, n, bk, bp, pk, pp)
 
 
@@ -123,17 +133,18 @@ def test_level2_overflow_in_one_parent(dj, oracle):
 def test_overflow_then_clean_call_on_one_workspace(dj, oracle):
     """Flags, cursors and capacities are rebuilt by every call: a clean join right after an
     overflowing one, in the same workspace, repairs nothing and is exact."""
-    _shape_a()
     rng = np.random.default_rng(5)
     ws = dj.workspace(dj.lib().dj_inner_join_workspace_bytes(NB, NB + NB // 4))
     bk = np.unique(_crowded(NB, rng))
     pk = _probe_for(bk, NB + NB // 4, rng, crowd=True)
+    want = _want(bk, pk, (2, 0))
     _repairs(dj)
     cols, n, bp, pp = _join(dj, bk, pk, ws)
-    assert _repairs(dj) == (2, 0)
+    assert _repairs(dj) == want
     _check(dj, oracle, cols, n, bk, bp, pk, pp)
     bk = np.unique(rng.integers(-(1 << 62), 1 << 62, NB))
     pk = _probe_for(bk, NB + NB // 4, rng, crowd=False)
+    assert _want(bk, pk, (0, 0)) == (0, 0)
     ws.fill_(-1)  # nothing from the earlier call may be needed
     cols, n, bp, pp = _join(dj, bk, pk, ws)
     assert _repairs(dj) == (0, 0)
@@ -146,19 +157,23 @@ def test_streamed_host_entry_with_overflowing_probe_chunk(dj, oracle):
     resident build buckets; only the second chunk is crowded, so exactly one level-1 pass repairs."""
     import torch
 
-    _shape_a()
     rng = np.random.default_rng(6)
     lk = np.unique(rng.integers(-(1 << 62), 1 << 62, NB))
     chunk = 1 << 20  # streamed_shape: 16 chunks, at least 1M rows each
     rk = np.concatenate([_probe_for(lk, chunk, rng, False), _probe_for(lk, chunk, rng, True),
                          _probe_for(lk, chunk // 2, rng, False)])
+    over = tagged(("build",), side_overflows(lk, BITS1, BITS2))
+    for c, at in enumerate(range(0, rk.size, chunk)):
+        over += tagged(("chunk", c), side_overflows(rk[at:at + chunk], BITS1, BITS2))
+    want = expected_repairs(over)
+    assert over == [("chunk", 1, 0, 0, HOT1)], over
     lp, rp = _ids(lk.size), _ids(rk.size, 1 << 40)
     ref_n, ref = oracle.inner_join(lk, lp, rk, rp)
     h_in = [torch.from_numpy(a).pin_memory() for a in (lk, lp, rk, rp)]
     h_out = [torch.empty(ref_n + 16, dtype=torch.int64).pin_memory() for _ in range(4)]
     _repairs(dj)
     n, _ = dj.distributed_inner_join_host(None, *h_in, h_out)
-    assert _repairs(dj) == (1, 0)
+    assert _repairs(dj) == want
     assert n == ref_n
     for a, b in zip(oracle.sort_rows(*[o[:n].numpy() for o in h_out]), oracle.sort_rows(*ref)):
         assert (a == b).all()
@@ -166,8 +181,7 @@ def test_streamed_host_entry_with_overflowing_probe_chunk(dj, oracle):
 
 @pytest.mark.gpu
 def test_generated_20m_join_repairs_nothing(dj, oracle):
-    """The benchmark's generator at 20M x 20M (two levels, 7 + 7 bits): no bucket reaches its capacity."""
-    _shape_a()
+    """The benchmark's generator at 20M x 20M (a two-level plan): no bucket reaches its capacity."""
     n = 20_000_000
     g = dj.gen_params(n, n, 0.3, 2 * n, True)
     bk, bp = dj.generate_rows(g, 0, 0, 0, n)
