@@ -102,7 +102,7 @@ RadixPlan plan_for(int64_t nbuild, bool /*any_segmented*/)
   return plan;
 }
 
-// A semi / anti join builds on the right table, which is often tiny next to the left one (a fact
+// A semi / anti / outer join builds on the right table, which is often tiny next to the left one (a fact
 // table filtered by a small key set).  The join kernel runs at most one CTA per bucket, so its
 // plan gets at least kFilterMinBits bits (1024 buckets: every SM busy with either CTA shape); a
 // bucket then holds less than one build job, and the probe side is spread over all of them.
@@ -237,7 +237,7 @@ int prepare_side(const TableInput& in, const RadixPlan& plan, PreparedSide* out,
 
 int join_prepared(const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
                   int64_t* const out[4], int64_t out_capacity, int64_t* d_out_count, bool swap,
-                  cudaStream_t stream, int kind, uint32_t* d_probe_bits)
+                  cudaStream_t stream, int kind, uint32_t* d_probe_bits, uint8_t* out_sides)
 {
   JoinBuffers jb{};
   jb.build = build.rows; jb.d_build_begin = build.d_begin; jb.d_build_end = build.d_end;
@@ -248,22 +248,43 @@ int join_prepared(const PreparedSide& build, const PreparedSide& probe, const Ra
   jb.d_out_count  = d_out_count;
   jb.kind         = kind;
   jb.d_probe_bits = d_probe_bits;
+  jb.out_sides    = out_sides;
   return run_bucket_join(jb, swap, stream);
+}
+
+// the zeroed probe-row bit array of a semi / anti / outer join (one bit per prepared probe row)
+static int zeroed_probe_bits(const PreparedSide& probe, Arena& arena, cudaStream_t stream, uint32_t** bits)
+{
+  const size_t words = (size_t)(probe.cap_rows + 31) / 32;
+  *bits              = arena.take<uint32_t>(words);
+  if (!*bits) {
+    set_error("join: workspace too small for the probe-row bits");
+    return DJ_ERR_WORKSPACE;
+  }
+  DJ_CUDA_TRY(cudaMemsetAsync(*bits, 0, words * 4, stream));
+  return DJ_OK;
 }
 
 int filter_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
                          int64_t* out_key, int64_t* out_pay, int64_t out_capacity, int64_t* d_out_count,
                          Arena& arena, cudaStream_t stream)
 {
-  const size_t words = (size_t)(probe.cap_rows + 31) / 32;
-  uint32_t* bits     = arena.take<uint32_t>(words);
-  if (!bits) {
-    set_error("left_filter_join: workspace too small");
-    return DJ_ERR_WORKSPACE;
-  }
-  DJ_CUDA_TRY(cudaMemsetAsync(bits, 0, words * 4, stream));
+  uint32_t* bits = nullptr;
+  int rc         = zeroed_probe_bits(probe, arena, stream, &bits);
+  if (rc) return rc;
   int64_t* const out[4] = {out_key, out_pay, nullptr, nullptr};
   return join_prepared(build, probe, plan, out, out_capacity, d_out_count, false, stream, kind, bits);
+}
+
+int outer_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
+                        int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
+                        Arena& arena, cudaStream_t stream)
+{
+  uint32_t* bits = nullptr;
+  int rc         = zeroed_probe_bits(probe, arena, stream, &bits);
+  if (rc) return rc;
+  // the kernel writes (build row, probe row) = (right, left): swapped into left ++ right
+  return join_prepared(build, probe, plan, out, out_capacity, d_out_count, true, stream, kind, bits, out_sides);
 }
 
 // Joins (bk,bp)[nb] with (pk,pp)[np]; appends matches at *d_out_count (running, device).
@@ -299,6 +320,20 @@ int local_filter_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl
   rc = prepare_side(tp, plan, &sp, arena, stream);
   if (rc) return rc;
   return filter_join_prepared(kind, sb, sp, plan, out_key, out_pay, out_capacity, d_out_count, arena, stream);
+}
+
+int local_outer_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* rk, const int64_t* rp,
+                     int64_t nr, int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
+                     Arena& arena, cudaStream_t stream)
+{
+  const RadixPlan plan = filter_plan(nr);
+  TableInput tb{rk, rp, nullptr, nr, nullptr, nullptr, 0}, tp{lk, lp, nullptr, nl, nullptr, nullptr, 0};
+  PreparedSide sb{}, sp{};
+  int rc = prepare_side(tb, plan, &sb, arena, stream);
+  if (rc) return rc;
+  rc = prepare_side(tp, plan, &sp, arena, stream);
+  if (rc) return rc;
+  return outer_join_prepared(kind, sb, sp, plan, out, out_sides, out_capacity, d_out_count, arena, stream);
 }
 
 }  // namespace dj

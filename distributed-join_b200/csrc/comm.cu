@@ -747,7 +747,8 @@ constexpr int kAlignRows = 32;
 
 static inline int64_t pad_rows(int64_t n) { return (n + kAlignRows - 1) / kAlignRows * kAlignRows; }
 
-// kind 0: inner join; DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI: semi / anti join (build side = right)
+// kind 0: inner join; any other kind (semi, anti, left / full outer) builds on the right table with
+// the filter plan and a probe-row bit array
 static size_t dist_ws_bytes(int64_t nl, int64_t nr, int world, int odf, double slack, int kind = 0)
 {
   if (world <= 1 && kind) return local_filter_join_workspace(nl, nr) + 8192;
@@ -831,13 +832,16 @@ static double ms_since(std::chrono::high_resolution_clock::time_point t0)
 // The distributed join of every kind.  kind 0: inner join, out = (left key, left payload, right key,
 // right payload).  DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI: the right table's key column is passed as its
 // payload too (d_right_payload == d_right_key), it is always the build side, and out[0..1] receive
-// the kept left rows (d_out_rk, d_out_rp are unused).
+// the kept left rows (d_out_rk, d_out_rp are unused).  DJ_JOIN_LEFT_OUTER / DJ_JOIN_FULL_OUTER: the
+// right table (with its payload) is always the build side, out as for the inner join, and
+// d_out_sides receives every row's DJ_SIDE_* bits.
 static int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key, const int64_t* d_left_payload,
                             int64_t nleft, const int64_t* d_right_key, const int64_t* d_right_payload,
                             int64_t nright, int64_t* d_out_lk, int64_t* d_out_lp, int64_t* d_out_rk,
-                            int64_t* d_out_rp, int64_t out_capacity, int64_t* h_out_count, dj_join_options* opts,
-                            void* d_workspace, size_t workspace_bytes, void* stream)
+                            int64_t* d_out_rp, uint8_t* d_out_sides, int64_t out_capacity, int64_t* h_out_count,
+                            dj_join_options* opts, void* d_workspace, size_t workspace_bytes, void* stream)
 {
+  const bool outer = kind == DJ_JOIN_LEFT_OUTER || kind == DJ_JOIN_FULL_OUTER;
   DJ_REQUIRE(nleft >= 0 && nright >= 0 && h_out_count && d_workspace, "distributed_inner_join: bad argument");
   cudaStream_t st   = (cudaStream_t)stream;
   const int world   = comm ? comm->size : 1;
@@ -862,7 +866,27 @@ static int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key
     // src/distributed_join.cpp:186-199 -- one rank: the local join is the whole job.
     const bool swap = kind == 0 && build_on_right(nleft, nright);
     int rc = DJ_OK;
-    if (kind == DJ_JOIN_LEFT_ANTI && nright == 0) {
+    // outer joins with one side empty: that side's rows are the result, the other side null
+    const bool outer_left_only  = outer && nright == 0 && nleft > 0;
+    const bool outer_right_only = kind == DJ_JOIN_FULL_OUTER && nleft == 0 && nright > 0;
+    if (outer_left_only || outer_right_only) {
+      const int64_t n = std::min(outer_left_only ? nleft : nright, out_capacity);
+      if (n > 0) {
+        int64_t* const present[2] = {outer_left_only ? d_out_lk : d_out_rk, outer_left_only ? d_out_lp : d_out_rp};
+        int64_t* const absent[2]  = {outer_left_only ? d_out_rk : d_out_lk, outer_left_only ? d_out_rp : d_out_lp};
+        DJ_CUDA_TRY(cudaMemcpyAsync(present[0], outer_left_only ? d_left_key : d_right_key, (size_t)n * 8,
+                                    cudaMemcpyDeviceToDevice, st));
+        DJ_CUDA_TRY(cudaMemcpyAsync(present[1], outer_left_only ? d_left_payload : d_right_payload, (size_t)n * 8,
+                                    cudaMemcpyDeviceToDevice, st));
+        DJ_CUDA_TRY(cudaMemsetAsync(absent[0], 0, (size_t)n * 8, st));
+        DJ_CUDA_TRY(cudaMemsetAsync(absent[1], 0, (size_t)n * 8, st));
+        DJ_CUDA_TRY(cudaMemsetAsync(d_out_sides, outer_left_only ? DJ_SIDE_LEFT : DJ_SIDE_RIGHT, (size_t)n, st));
+      }
+    } else if (outer) {
+      if (nleft > 0 && nright > 0)
+        rc = local_outer_join(kind, d_left_key, d_left_payload, nleft, d_right_key, d_right_payload, nright, out,
+                              d_out_sides, out_capacity, d_count, arena, st);
+    } else if (kind == DJ_JOIN_LEFT_ANTI && nright == 0) {
       // nothing to match: the anti join keeps every left row
       const int64_t n = std::min(nleft, out_capacity);
       if (n > 0) {
@@ -885,6 +909,8 @@ static int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key
     DJ_CUDA_TRY(cudaStreamSynchronize(st));
     if (comm) *h_out_count = comm->h_pinned[0];
     if (kind == DJ_JOIN_LEFT_ANTI && nright == 0) *h_out_count = nleft;
+    if (outer_left_only) *h_out_count = nleft;
+    if (outer_right_only) *h_out_count = nright;
     if (timing) {
       opts->t_join_ms = ms_since(t0);
       // the reference labels this branch's time "Hash partition" (src/distributed_join.cpp:194)
@@ -1415,6 +1441,21 @@ static int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key
           return rc;
         }
       }
+      // outer joins: the received rows of the non-empty side, with the other side null
+      for (int t = 0; t < 2 && outer; t++) {
+        const Piece& pc = t ? R : L;
+        if (pc.rows == 0 || (t == 1 && kind != DJ_JOIN_FULL_OUTER)) continue;
+        int64_t longest = 0;
+        for (int s = 0; s < G; s++) longest = std::max(longest, pc.count[s]);
+        rc = t ? append_segment_rows(R.data, R.d_seg_begin, R.d_seg_end, nseg, longest, d_out_rk, d_out_rp,
+                                     out_capacity, d_count, st, d_out_lk, d_out_lp, d_out_sides, DJ_SIDE_RIGHT)
+               : append_segment_rows(L.data, L.d_seg_begin, L.d_seg_end, nseg, longest, d_out_lk, d_out_lp,
+                                     out_capacity, d_count, st, d_out_rk, d_out_rp, d_out_sides, DJ_SIDE_LEFT);
+        if (rc) {
+          drain_exchange();
+          return rc;
+        }
+      }
       continue;
     }
     const bool swap = kind == 0 && build_on_right(L.rows, R.rows);
@@ -1437,8 +1478,9 @@ static int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key
       }
       trace.mark(t ? "radix(R) end" : "radix(L) end", st);
     }
-    rc = kind ? filter_join_prepared(kind, side[1], side[0], plan, d_out_lk, d_out_lp, out_capacity, d_count, arena, st)
-              : join_prepared(side[swap ? 1 : 0], side[swap ? 0 : 1], plan, out, out_capacity, d_count, swap, st);
+    rc = outer  ? outer_join_prepared(kind, side[1], side[0], plan, out, d_out_sides, out_capacity, d_count, arena, st)
+         : kind ? filter_join_prepared(kind, side[1], side[0], plan, d_out_lk, d_out_lp, out_capacity, d_count, arena, st)
+                : join_prepared(side[swap ? 1 : 0], side[swap ? 0 : 1], plan, out, out_capacity, d_count, swap, st);
     if (rc) {
       drain_exchange();
       return rc;
@@ -1547,8 +1589,8 @@ extern "C" int dj_distributed_inner_join_i64(dj_comm_t* comm, const int64_t* d_l
                                              size_t workspace_bytes, void* stream)
 {
   return distributed_join(comm, 0, d_left_key, d_left_payload, nleft, d_right_key, d_right_payload, nright, d_out_lk,
-                          d_out_lp, d_out_rk, d_out_rp, out_capacity, h_out_count, opts, d_workspace, workspace_bytes,
-                          stream);
+                          d_out_lp, d_out_rk, d_out_rp, nullptr, out_capacity, h_out_count, opts, d_workspace,
+                          workspace_bytes, stream);
 }
 
 extern "C" size_t dj_distributed_left_filter_join_workspace_bytes(int64_t nleft, int64_t nright, int world,
@@ -1568,8 +1610,32 @@ extern "C" int dj_distributed_left_filter_join_i64(dj_comm_t* comm, int kind, co
   DJ_REQUIRE(out_capacity >= 0 && (out_capacity == 0 || (d_out_key && d_out_payload)),
              "left_filter_join: bad output columns");
   return distributed_join(comm, kind, d_left_key, d_left_payload, nleft, d_right_key, d_right_key, nright, d_out_key,
-                          d_out_payload, nullptr, nullptr, out_capacity, h_out_count, opts, d_workspace,
+                          d_out_payload, nullptr, nullptr, nullptr, out_capacity, h_out_count, opts, d_workspace,
                           workspace_bytes, stream);
+}
+
+// An outer join needs what a semi / anti join needs: the same plan, padded sides and probe-row bits
+// (the right table's payload travels in the rows either way).
+extern "C" size_t dj_distributed_outer_join_workspace_bytes(int64_t nleft, int64_t nright, int world,
+                                                            int over_decom_factor)
+{
+  return dist_ws_bytes(nleft, nright, world, over_decom_factor < 1 ? 1 : over_decom_factor, 1.15, DJ_JOIN_LEFT_OUTER);
+}
+
+extern "C" int dj_distributed_outer_join_i64(dj_comm_t* comm, int kind, const int64_t* d_left_key,
+                                             const int64_t* d_left_payload, int64_t nleft,
+                                             const int64_t* d_right_key, const int64_t* d_right_payload,
+                                             int64_t nright, int64_t* d_out_lk, int64_t* d_out_lp,
+                                             int64_t* d_out_rk, int64_t* d_out_rp, uint8_t* d_out_sides,
+                                             int64_t out_capacity, int64_t* h_out_count, dj_join_options* opts,
+                                             void* d_workspace, size_t workspace_bytes, void* stream)
+{
+  DJ_REQUIRE(kind == DJ_JOIN_LEFT_OUTER || kind == DJ_JOIN_FULL_OUTER, "outer_join: unknown join kind %d", kind);
+  DJ_REQUIRE(out_capacity >= 0 && (out_capacity == 0 || (d_out_lk && d_out_lp && d_out_rk && d_out_rp && d_out_sides)),
+             "outer_join: bad output columns");
+  return distributed_join(comm, kind, d_left_key, d_left_payload, nleft, d_right_key, d_right_payload, nright,
+                          d_out_lk, d_out_lp, d_out_rk, d_out_rp, d_out_sides, out_capacity, h_out_count, opts,
+                          d_workspace, workspace_bytes, stream);
 }
 
 static size_t streamed_ws_bytes(int64_t nleft, int64_t nright, int64_t out_capacity);

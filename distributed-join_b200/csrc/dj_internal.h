@@ -144,15 +144,20 @@ struct JoinBuffers {
   int64_t* d_out_count;    // running total (device); the kernel atomically adds to it
   // 0: inner join.  DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI: the build side is the right table, out[0..1]
   // receive the probe (left) rows, and d_probe_bits holds one zeroed bit per row of `probe`.
+  // DJ_JOIN_LEFT_OUTER / DJ_JOIN_FULL_OUTER: the build side is the right table, d_probe_bits as for
+  // semi / anti, and out_sides receives every output row's DJ_SIDE_* bits.
   int kind               = 0;
   uint32_t* d_probe_bits = nullptr;
+  uint8_t* out_sides     = nullptr;
 };
 int run_bucket_join(const JoinBuffers& jb, bool swap_output_sides, cudaStream_t stream);
 // Appends the rows of segments [d_seg_begin[i], d_seg_end[i]) (each at most max_seg_rows long) to
-// (out_key, out_pay) at the running count *d_out_count, in no particular order.
+// (out_key, out_pay) at the running count *d_out_count, in no particular order.  With out_sides set
+// (outer joins), the same output rows of (null_key, null_pay) are zeroed and their sides byte is set.
 int append_segment_rows(const Row* rows, const int64_t* d_seg_begin, const int64_t* d_seg_end, int nseg,
                         int64_t max_seg_rows, int64_t* out_key, int64_t* out_pay, int64_t out_capacity,
-                        int64_t* d_out_count, cudaStream_t stream);
+                        int64_t* d_out_count, cudaStream_t stream, int64_t* null_key = nullptr,
+                        int64_t* null_pay = nullptr, uint8_t* out_sides = nullptr, uint8_t sides = 0);
 
 // Radix plan for a local join with `nbuild` build rows.
 struct RadixPlan {
@@ -185,7 +190,7 @@ struct PreparedSide {
 };
 RadixPlan plan_for(int64_t nbuild, bool any_segmented);
 size_t side_ws_bytes(int64_t span_rows, const RadixPlan& plan, int nseg);
-// Semi / anti joins: the plan for `nright` build rows with at least kFilterMinBits bits, so that the
+// Semi / anti / outer joins: the plan for `nright` build rows with at least kFilterMinBits bits, so that the
 // probe side is spread over every SM however small the right table is; and the bytes of the
 // probe-row bit array for a probe side spanning `span_rows` rows.
 constexpr int kFilterMinBits = 10;
@@ -214,12 +219,19 @@ int prepare_side(const TableInput& in, const RadixPlan& plan, PreparedSide* out,
                  cudaStream_t stream);
 int join_prepared(const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
                   int64_t* const out[4], int64_t out_capacity, int64_t* d_out_count, bool swap,
-                  cudaStream_t stream, int kind = 0, uint32_t* d_probe_bits = nullptr);
+                  cudaStream_t stream, int kind = 0, uint32_t* d_probe_bits = nullptr,
+                  uint8_t* out_sides = nullptr);
 // Semi / anti join of the probe side's rows against the build side's keys: zeroes the probe-row
 // bit array (taken from `arena`) and runs the join kernel of that kind; out = (key, payload).
 int filter_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
                          int64_t* out_key, int64_t* out_pay, int64_t out_capacity, int64_t* d_out_count,
                          Arena& arena, cudaStream_t stream);
+// Left / full outer join of the probe (left) side against the build (right) side: zeroes the
+// probe-row bit array (taken from `arena`) and runs the join kernel of that kind.  out = (left key,
+// left payload, right key, right payload), out_sides = DJ_SIDE_* bits of every row.
+int outer_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
+                        int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
+                        Arena& arena, cudaStream_t stream);
 int local_join(const int64_t* bk, const int64_t* bp, int64_t nb, const int64_t* pk,
                const int64_t* pp, int64_t np, int64_t* const out[4], int64_t out_capacity,
                int64_t* d_out_count, bool swap, Arena& arena, cudaStream_t stream);
@@ -229,6 +241,11 @@ int local_filter_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl
                       int64_t* out_key, int64_t* out_pay, int64_t out_capacity, int64_t* d_out_count, Arena& arena,
                       cudaStream_t stream);
 size_t local_filter_join_workspace(int64_t nl, int64_t nr);
+// Single-GPU left / full outer join of (lk, lp)[nl] with (rk, rp)[nr]; both sides non-empty.  Its
+// workspace is local_filter_join_workspace(nl, nr): the same plan, sides and probe-row bits.
+int local_outer_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* rk, const int64_t* rp,
+                     int64_t nr, int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
+                     Arena& arena, cudaStream_t stream);
 
 // One kernel of each translation unit's module (partition.cu, join.cu, generate.cu): comm.cu
 // loads every function of these modules before ranks can wait on each other.

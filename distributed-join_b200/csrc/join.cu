@@ -33,7 +33,18 @@
 // The jobs of a bucket run in order in one CTA, and the consumer barrier between two jobs orders
 // the bit updates.  An anti join also runs one (empty) build job for a bucket whose build side is
 // empty, so that its probe rows are all emitted.
+//
+// Left / full outer joins (KIND = DJ_JOIN_LEFT_OUTER / DJ_JOIN_FULL_OUTER) also build on the right
+// table.  The probe loop is the inner join's multimap loop; each lane also remembers whether its row
+// matched in this job, and the anti join's bit rule decides, in a bucket's last job, which probe rows
+// matched nothing: those are emitted once with an absent build side.  A full outer join keeps one bit
+// per staged build row in shared memory (set on every match); every probe row of the bucket streams
+// past every build job, so at the end of a job the build rows with a clear bit are exactly the right
+// rows without a match, and they are emitted with an absent probe side.  Output tiles of these kinds
+// carry a sides byte next to the four columns (bit 0: probe / left row present, bit 1: build / right
+// row present); absent columns are written as 0.
 #include <cstdlib>
+#include <type_traits>
 
 #include "dj_device.cuh"
 #include "dj_internal.h"
@@ -71,10 +82,17 @@ struct JoinDev {
   int64_t* out[4];
   int64_t out_capacity;
   unsigned long long* out_count;
-  uint32_t* probe_bits;  // semi / anti: one bit per row of `probe` (multi-job buckets only)
+  uint32_t* probe_bits;  // semi / anti / outer: one bit per row of `probe` (multi-job buckets only)
+  uint8_t* out_sides;    // outer joins: DJ_SIDE_* bits of every output row
 };
 
 constexpr int kInner = 0, kSemi = DJ_JOIN_LEFT_SEMI, kAnti = DJ_JOIN_LEFT_ANTI;
+constexpr int kLeftOuter = DJ_JOIN_LEFT_OUTER, kFullOuter = DJ_JOIN_FULL_OUTER;
+// sides byte of an outer join's output row, in the kernel's (build, probe) terms: the probe side is
+// the left table, the build side the right one
+constexpr uint8_t kSideProbe = DJ_SIDE_LEFT, kSideBuild = DJ_SIDE_RIGHT;
+
+__host__ __device__ constexpr bool is_outer(int kind) { return kind == kLeftOuter || kind == kFullOuter; }
 
 template <class C>
 struct __align__(128) JoinSmem {
@@ -90,6 +108,17 @@ struct __align__(128) JoinSmem {
   int scnt[kOutTiles];
 };
 
+// Outer joins: the output tiles' sides bytes, and (full outer) one "matched" bit per staged build
+// row of each of the two tables.
+template <class C>
+struct __align__(128) OuterJoinSmem : JoinSmem<C> {
+  uint8_t ssides[kOutTiles][C::kOutRows];
+  uint32_t bmatch[2][C::kBuildChunk / 32];
+};
+
+template <class C, int KIND>
+using JoinSmemOf = std::conditional_t<is_outer(KIND), OuterJoinSmem<C>, JoinSmem<C>>;
+
 template <int N>
 __device__ __forceinline__ void consumer_sync()
 {
@@ -97,12 +126,15 @@ __device__ __forceinline__ void consumer_sync()
 }
 
 // Build jobs of the cached descriptor block: (bucket, build chunk) pairs whose bucket is
-// non-empty on both sides (anti: on the probe side).  Every thread walks them identically.
+// non-empty on both sides (anti, left outer: on the probe side; full outer: on either side).
+// Every thread walks them identically.
 template <int KIND, class S>
 __device__ __forceinline__ int next_valid_bucket(const S& s, int lb, int nd)
 {
-  if constexpr (KIND == kAnti) {
+  if constexpr (KIND == kAnti || KIND == kLeftOuter) {
     while (lb < nd && s.dpe[lb] == s.dpb[lb]) lb++;
+  } else if constexpr (KIND == kFullOuter) {
+    while (lb < nd && s.dbe[lb] == s.dbb[lb] && s.dpe[lb] == s.dpb[lb]) lb++;
   } else {
     while (lb < nd && (s.dbe[lb] == s.dbb[lb] || s.dpe[lb] == s.dpb[lb])) lb++;
   }
@@ -112,12 +144,59 @@ __device__ __forceinline__ int next_valid_bucket(const S& s, int lb, int nd)
 // Slot word: bit 31 = occupied, bits 30..11 = 20-bit key fingerprint, bits 10..0 = build row.
 __device__ __forceinline__ uint32_t slot_tag(uint32_t h) { return 0x100000u | (h >> 12); }
 
+// Outer joins: every lane with `emit` set appends the row (bk, bp, pk, pv, sides) to output tile
+// `cur`; once the tile is full, the warp reserves its own run of the output and stores the rest
+// directly.  Called by all 32 lanes of a warp.
+template <class C>
+__device__ __forceinline__ void emit_outer_row(OuterJoinSmem<C>& s, const JoinDev& d, int cur, int lane, bool emit,
+                                               int64_t bk, int64_t bp, int64_t pk, int64_t pv, uint8_t sides)
+{
+  const unsigned m = __ballot_sync(0xffffffffu, emit);
+  if (m == 0) return;
+  const int leader = __ffs(m) - 1;
+  int obase        = 0;
+  if (lane == leader) {
+    obase = atomicAdd(&s.scnt[cur], __popc(m));
+    if (obase >= C::kOutRows) atomicSub(&s.scnt[cur], __popc(m));  // a full tile stays full (see inner)
+  }
+  obase            = __shfl_sync(0xffffffffu, obase, leader);
+  const int pos    = obase + __popc(m & lanemask_lt());
+  const bool spill = emit && pos >= C::kOutRows;
+  if (emit && !spill) {
+    s.sout[cur][0][pos] = bk;
+    s.sout[cur][1][pos] = bp;
+    s.sout[cur][2][pos] = pk;
+    s.sout[cur][3][pos] = pv;
+    s.ssides[cur][pos]  = sides;
+  }
+  const unsigned ms = __ballot_sync(0xffffffffu, spill);
+  if (ms) {
+    const int sl         = __ffs(ms) - 1;
+    unsigned long long g = 0;
+    if (lane == sl) g = atomicAdd(d.out_count, (unsigned long long)__popc(ms));
+    g = __shfl_sync(0xffffffffu, g, sl);
+    if (spill) {
+      const int64_t gi = (int64_t)g + __popc(ms & lanemask_lt());
+      if (gi < d.out_capacity) {
+        d.out[0][gi]     = bk;
+        d.out[1][gi]     = bp;
+        d.out[2][gi]     = pk;
+        d.out[3][gi]     = pv;
+        d.out_sides[gi]  = sides;
+      }
+    }
+  }
+}
+
 template <class C, int KIND>
 __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
 {
-  using Smem = JoinSmem<C>;
+  using Smem = JoinSmemOf<C, KIND>;
   constexpr int kConsumers = C::kConsumers;
-  constexpr int kCols      = KIND == kInner ? 4 : 2;  // output columns
+  constexpr bool kOuter    = is_outer(KIND);
+  // a bucket with probe rows but no build rows still runs one (empty) build job
+  constexpr bool kEmptyJob = KIND == kAnti || kOuter;
+  constexpr int kCols      = (KIND == kSemi || KIND == kAnti) ? 2 : 4;  // output columns
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& s        = *reinterpret_cast<Smem*>(smem_raw);
   const int tid  = threadIdx.x;
@@ -138,6 +217,8 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int i = tid; i < 2 * C::kSlots; i += C::kThreads) (&s.slots[0][0])[i] = 0;
+  if constexpr (KIND == kFullOuter)
+    for (int i = tid; i < 2 * (C::kBuildChunk / 32); i += C::kThreads) (&s.bmatch[0][0])[i] = 0;
   __syncthreads();
 
   // contiguous bucket range of this CTA
@@ -167,13 +248,13 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
       if (lane == 0) {
         for (int lb = next_valid_bucket<KIND>(s, 0, nd); lb < nd; lb = next_valid_bucket<KIND>(s, lb + 1, nd)) {
           const int64_t b0 = s.dbb[lb], b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
-          for (int64_t c0 = b0; c0 < b1 || (KIND == kAnti && c0 == b0); c0 += C::kBuildChunk) {
+          for (int64_t c0 = b0; c0 < b1 || (kEmptyJob && c0 == b0); c0 += C::kBuildChunk) {
             {
               const int bs = u & 1;
-              const int n  = (int)min((int64_t)C::kBuildChunk, b1 - c0);  // anti: 0 for an empty build side
+              const int n  = (int)min((int64_t)C::kBuildChunk, b1 - c0);  // 0 for an empty build job
               mbar_wait(&s.empty_build[bs], ((u >> 1) & 1) ^ 1);
               mbar_expect_tx(&s.full_build[bs], (uint32_t)n * 16u);
-              if (KIND != kAnti || n > 0) tma_load(s.brow[bs], d.build + c0, (uint32_t)n * 16u, &s.full_build[bs]);
+              if (!kEmptyJob || n > 0) tma_load(s.brow[bs], d.build + c0, (uint32_t)n * 16u, &s.full_build[bs]);
               u++;
             }
             for (int64_t r0 = p0; r0 < p1; r0 += C::kProbeChunk) {
@@ -192,9 +273,9 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
       // ------------------------------------------------------------ consumers
       for (int lb = next_valid_bucket<KIND>(s, 0, nd); lb < nd; lb = next_valid_bucket<KIND>(s, lb + 1, nd)) {
         const int64_t b0 = s.dbb[lb], b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
-        // semi / anti: does this bucket's build side span several jobs, and is this its last job
+        // semi / anti / outer: does this bucket's build side span several jobs, and is this its last job
         const bool multi = KIND != kInner && b1 - b0 > C::kBuildChunk;
-        for (int64_t c0 = b0; c0 < b1 || (KIND == kAnti && c0 == b0); c0 += C::kBuildChunk) {
+        for (int64_t c0 = b0; c0 < b1 || (kEmptyJob && c0 == b0); c0 += C::kBuildChunk) {
           const bool last = c0 + C::kBuildChunk >= b1;
           // ---- build: fingerprint + row index into a 32-bit slot claimed with atomicCAS; the
           //      staged rows themselves are the row store (no copy)
@@ -213,6 +294,8 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
           {
             uint4* other = reinterpret_cast<uint4*>(s.slots[bs ^ 1]);
             for (int i = tid; i < C::kSlots / 4; i += kConsumers) other[i] = make_uint4(0, 0, 0, 0);
+            if constexpr (KIND == kFullOuter)
+              for (int i = tid; i < C::kBuildChunk / 32; i += kConsumers) s.bmatch[bs ^ 1][i] = 0;
           }
           consumer_sync<kConsumers>();  // table complete
 
@@ -243,7 +326,54 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
             const uint32_t h    = slot_hash_i64(k);
             const uint32_t want = slot_tag(h);
             uint32_t slot       = h & (C::kSlots - 1);
-            if constexpr (KIND != kInner) {
+            if constexpr (kOuter) {
+              // outer: the inner join's multimap walk, remembering whether this row matched at all
+              const bool valid = alive;
+              bool matched     = false;
+              while (true) {
+                bool found = false;
+                int idx    = 0;
+                if (alive) {
+                  while (true) {
+                    const uint32_t e = slots[slot];
+                    if (e == 0u) {
+                      alive = false;
+                      break;
+                    }
+                    if ((e >> 11) == want) {
+                      idx = (int)(e & 0x7ffu);
+                      if (brow[idx].key == k) {
+                        found = true;
+                        break;
+                      }
+                    }
+                    slot = (slot + 1) & (C::kSlots - 1);
+                  }
+                }
+                if (!__any_sync(0xffffffffu, found)) break;
+                int64_t bpay = 0;
+                if (found) {
+                  matched = true;
+                  bpay    = brow[idx].pay;
+                  if constexpr (KIND == kFullOuter) {
+                    uint32_t* w      = &s.bmatch[bs][idx >> 5];
+                    const uint32_t b = 1u << (idx & 31);
+                    if (!(*w & b)) atomicOr(w, b);
+                  }
+                }
+                emit_outer_row<C>(s, d, cur, lane, found, k, bpay, k, v, kSideBuild | kSideProbe);
+                if (found) slot = (slot + 1) & (C::kSlots - 1);  // multimap: scan past the hit
+              }
+              // the anti join's rule: a row is unmatched when no job of its bucket matched it
+              const int64_t prow_at = r0 + tid;
+              uint32_t* word        = d.probe_bits + (prow_at >> 5);
+              const uint32_t bit    = 1u << (prow_at & 31);
+              if (multi && matched && !last) atomicOr(word, bit);
+              const bool lone = valid && !matched && last && (!multi || !(__ldcg(word) & bit));
+              emit_outer_row<C>(s, d, cur, lane, lone, 0, 0, k, v, kSideProbe);
+              continue;
+            }
+            if constexpr (KIND == kSemi || KIND == kAnti) {
               // semi / anti: walk to the first key match or to the end of the cluster
               bool found = false;
               if (alive) {
@@ -365,6 +495,22 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
           // ---- end of build job: table and row store are released, output tiles rotate
           if (tid == 0 && pend_n) s.sbase[pend_tile] = pend_base_reg;
           consumer_sync<kConsumers>();
+          if constexpr (KIND == kFullOuter) {
+            // every probe row of the bucket has passed this job: its build rows with a clear bit match
+            // no left row.  They are read from the row store and appended to tile `cur`, so the store
+            // is released and the tile handed over only after a second barrier.
+            for (int r0 = tid - lane; r0 < nb; r0 += kConsumers) {
+              const int r     = r0 + lane;
+              const bool lone = r < nb && !((s.bmatch[bs][r >> 5] >> (r & 31)) & 1u);
+              int64_t bk = 0, bp = 0;
+              if (lone) {
+                bk = brow[r].key;
+                bp = brow[r].pay;
+              }
+              emit_outer_row<C>(s, d, cur, lane, lone, bk, bp, 0, 0, kSideBuild);
+            }
+            consumer_sync<kConsumers>();
+          }
           if (lane == 0) mbar_arrive(&s.empty_build[bs]);
           if (pend_n) {
             // copy out the tile whose atomicAdd was issued one build job ago (latency hidden);
@@ -374,6 +520,9 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
             for (int c = 0; c < kCols; c++)
               for (int i = tid; i < pend_n; i += kConsumers)
                 if (gb + i < d.out_capacity) d.out[c][gb + i] = s.sout[pend_tile][c][i];
+            if constexpr (kOuter)
+              for (int i = tid; i < pend_n; i += kConsumers)
+                if (gb + i < d.out_capacity) d.out_sides[gb + i] = s.ssides[pend_tile][i];
             if (tid == 0) s.scnt[pend_tile] = 0;
             pend_n = 0;
           }
@@ -401,6 +550,9 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
       for (int c = 0; c < kCols; c++)
         for (int i = tid; i < pend_n; i += kConsumers)
           if (gb + i < d.out_capacity) d.out[c][gb + i] = s.sout[pend_tile][c][i];
+      if constexpr (kOuter)
+        for (int i = tid; i < pend_n; i += kConsumers)
+          if (gb + i < d.out_capacity) d.out_sides[gb + i] = s.ssides[pend_tile][i];
     }
   }
 }
@@ -418,7 +570,7 @@ int join_shape()
 template <class C, int KIND>
 int launch_join(const JoinDev& d, int ctas_per_sm, cudaStream_t stream)
 {
-  const size_t smem = sizeof(JoinSmem<C>);
+  const size_t smem = sizeof(JoinSmemOf<C, KIND>);
   auto kern         = bucket_join_kernel<C, KIND>;
   DJ_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = sm_count() * ctas_per_sm;
@@ -434,18 +586,22 @@ int launch_join(const JoinDev& d, int ctas_per_sm, cudaStream_t stream)
 template <class C>
 int launch_join_kind(const JoinDev& d, int kind, int ctas_per_sm, cudaStream_t stream)
 {
-  return kind == kSemi   ? launch_join<C, kSemi>(d, ctas_per_sm, stream)
-         : kind == kAnti ? launch_join<C, kAnti>(d, ctas_per_sm, stream)
-                         : launch_join<C, kInner>(d, ctas_per_sm, stream);
+  return kind == kSemi        ? launch_join<C, kSemi>(d, ctas_per_sm, stream)
+         : kind == kAnti      ? launch_join<C, kAnti>(d, ctas_per_sm, stream)
+         : kind == kLeftOuter ? launch_join<C, kLeftOuter>(d, ctas_per_sm, stream)
+         : kind == kFullOuter ? launch_join<C, kFullOuter>(d, ctas_per_sm, stream)
+                              : launch_join<C, kInner>(d, ctas_per_sm, stream);
 }
 
-// Appends the rows of segments [sb[i], se[i]) of `rows` (blockIdx.y = segment) to a two-column
-// output at the running count: an anti join's probe rows when the build side is empty.
+// Appends the rows of segments [sb[i], se[i]) of `rows` (blockIdx.y = segment) to (out_key, out_pay)
+// at the running count: an anti or outer join's rows whose other side is empty in this batch.  Outer
+// joins also zero the absent side's columns (null_key, null_pay) and set the rows' sides byte.
 constexpr int kAppendChunk = 4096;  // rows per output reservation
 
 __global__ void __launch_bounds__(256) append_rows_kernel(const Row* rows, const int64_t* sb, const int64_t* se,
-                                                          int64_t* out_key, int64_t* out_pay, int64_t out_capacity,
-                                                          unsigned long long* out_count)
+                                                          int64_t* out_key, int64_t* out_pay, int64_t* null_key,
+                                                          int64_t* null_pay, uint8_t* out_sides, uint8_t sides,
+                                                          int64_t out_capacity, unsigned long long* out_count)
 {
   __shared__ unsigned long long base;
   const int64_t b = sb[blockIdx.y], e = se[blockIdx.y];
@@ -460,6 +616,11 @@ __global__ void __launch_bounds__(256) append_rows_kernel(const Row* rows, const
         const Row r = rows[c0 + i];
         out_key[g]  = r.key;
         out_pay[g]  = r.pay;
+        if (out_sides) {
+          null_key[g]  = 0;
+          null_pay[g]  = 0;
+          out_sides[g] = sides;
+        }
       }
     }
   }
@@ -498,21 +659,23 @@ int run_bucket_join(const JoinBuffers& jb, bool swap_output_sides, cudaStream_t 
   d.out_capacity = jb.out_capacity;
   d.out_count    = (unsigned long long*)jb.d_out_count;
   d.probe_bits   = jb.d_probe_bits;
+  d.out_sides    = jb.out_sides;
   return join_shape() == 1 ? launch_join_kind<CfgB>(d, jb.kind, 2, stream)
                            : launch_join_kind<CfgA>(d, jb.kind, 1, stream);
 }
 
 int append_segment_rows(const Row* rows, const int64_t* d_seg_begin, const int64_t* d_seg_end, int nseg,
                         int64_t max_seg_rows, int64_t* out_key, int64_t* out_pay, int64_t out_capacity,
-                        int64_t* d_out_count, cudaStream_t stream)
+                        int64_t* d_out_count, cudaStream_t stream, int64_t* null_key, int64_t* null_pay,
+                        uint8_t* out_sides, uint8_t sides)
 {
   if (nseg <= 0 || max_seg_rows <= 0) return DJ_OK;
   const int64_t chunks = (max_seg_rows + kAppendChunk - 1) / kAppendChunk;
   const dim3 grid((unsigned)(chunks < 64 ? chunks : 64), (unsigned)nseg);
   {
     ProfScope prof(DJ_PROF_OTHER, stream);
-    append_rows_kernel<<<grid, 256, 0, stream>>>(rows, d_seg_begin, d_seg_end, out_key, out_pay, out_capacity,
-                                                 (unsigned long long*)d_out_count);
+    append_rows_kernel<<<grid, 256, 0, stream>>>(rows, d_seg_begin, d_seg_end, out_key, out_pay, null_key, null_pay,
+                                                 out_sides, sides, out_capacity, (unsigned long long*)d_out_count);
   }
   DJ_LAUNCH_CHECK();
   return DJ_OK;

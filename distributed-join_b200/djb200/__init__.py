@@ -29,6 +29,10 @@ ERR_OVERFLOW = 5
 
 JOIN_LEFT_SEMI = 1
 JOIN_LEFT_ANTI = 2
+JOIN_LEFT_OUTER = 3
+JOIN_FULL_OUTER = 4
+SIDE_LEFT = 1  # bits of an outer join's `sides` column: which side of an output row is present
+SIDE_RIGHT = 2
 
 
 class DjError(RuntimeError):
@@ -77,6 +81,7 @@ ABI_SYMBOLS = [
     "dj_distributed_inner_join_i64", "dj_distributed_inner_join_host_workspace_bytes",
     "dj_distributed_inner_join_i64_host", "dj_comm_create_local_group", "dj_testing_radix_repairs",
     "dj_distributed_left_filter_join_workspace_bytes", "dj_distributed_left_filter_join_i64",
+    "dj_distributed_outer_join_workspace_bytes", "dj_distributed_outer_join_i64",
 ]
 
 _lib = None
@@ -133,6 +138,10 @@ def lib() -> C.CDLL:
     L.dj_distributed_left_filter_join_workspace_bytes.argtypes = [i64, i64, C.c_int, C.c_int]
     L.dj_distributed_left_filter_join_i64.argtypes = [vp, C.c_int, vp, vp, i64, vp, i64, vp, vp, i64, C.POINTER(i64),
                                                       C.POINTER(JoinOptions), vp, sz, vp]
+    L.dj_distributed_outer_join_workspace_bytes.restype = sz
+    L.dj_distributed_outer_join_workspace_bytes.argtypes = [i64, i64, C.c_int, C.c_int]
+    L.dj_distributed_outer_join_i64.argtypes = [vp, C.c_int, vp, vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, i64,
+                                                C.POINTER(i64), C.POINTER(JoinOptions), vp, sz, vp]
     L.dj_comm_create_local_group.argtypes = [C.c_int, C.POINTER(vp)]
     L.dj_testing_radix_repairs.argtypes = [C.POINTER(i64)]
     _lib = L
@@ -353,9 +362,19 @@ class Comm:
 
 @dataclass
 class JoinResult:
-    cols: tuple  # (left key, left payload, right key, right payload), trimmed
+    cols: tuple  # (left key, left payload, right key, right payload[, sides]), trimmed
     n_out: int
     options: JoinOptions
+
+    @property
+    def sides(self):
+        """Outer joins: the uint8 SIDE_LEFT / SIDE_RIGHT bits of every row (None for other joins)."""
+        return self.cols[4] if len(self.cols) == 5 else None
+
+
+def _out_columns(ncols, capacity, dev):
+    """Output columns of one attempt: int64, and a fifth (an outer join's sides) of uint8."""
+    return [torch.empty(capacity, dtype=torch.uint8 if c == 4 else torch.int64, device=dev) for c in range(ncols)]
 
 
 def _collective_join(comm, call, ncols, capacity, ws, ws_bytes, outs, dev):
@@ -367,7 +386,7 @@ def _collective_join(comm, call, ncols, capacity, ws, ws_bytes, outs, dev):
         ws = workspace(ws_bytes, dev)
     while True:
         if outs is None or outs[0].numel() < capacity:
-            outs = [torch.empty(capacity, dtype=torch.int64, device=dev) for _ in range(ncols)]
+            outs = _out_columns(ncols, capacity, dev)
         rc, n, opts = call(outs, capacity, ws)
         _check(rc, allow=(ERR_OVERFLOW, ERR_WORKSPACE) if world > 1 else (ERR_OVERFLOW,))
         if rc == 0:
@@ -383,7 +402,7 @@ def _collective_join(comm, call, ncols, capacity, ws, ws_bytes, outs, dev):
         # every rank must retry together: agree on the largest need
         need = max(comm.allgather_i64([n])) if comm and comm.size > 1 else n
         capacity = need
-        outs = [torch.empty(capacity, dtype=torch.int64, device=dev) for _ in range(ncols)]
+        outs = _out_columns(ncols, capacity, dev)
         if comm and comm.size > 1:
             comm.barrier()
 
@@ -442,6 +461,42 @@ def distributed_left_semi_join(comm, lk, lp, rk, odf=1, capacity=None, ws=None, 
 def distributed_left_anti_join(comm, lk, lp, rk, odf=1, capacity=None, ws=None, outs=None):
     """Every left row whose key does not appear in rk (NOT EXISTS / NOT IN): see distributed_left_filter_join."""
     return distributed_left_filter_join(comm, JOIN_LEFT_ANTI, lk, lp, rk, odf, capacity, ws, outs)
+
+
+def distributed_outer_join(comm, kind, lk, lp, rk, rp, odf=1, capacity=None, ws=None, outs=None):
+    """Left outer (kind JOIN_LEFT_OUTER) or full outer (JOIN_FULL_OUTER) join of (lk, lp) with (rk, rp)
+    through dj_distributed_outer_join_i64.  Returns a JoinResult whose cols are (left key, left payload,
+    right key, right payload, sides), trimmed: sides (uint8) holds SIDE_LEFT | SIDE_RIGHT for a matched
+    pair, SIDE_LEFT for a left row without a match, SIDE_RIGHT (full outer) for a right row without
+    one; the absent side's columns are 0.  At N > 1 the rows whose keys this rank owns.  `outs`: four
+    int64 columns and one uint8 column, caller-owned, for the first attempt."""
+    lk, lp, rk, rp = map(_i64dev, (lk, lp, rk, rp))
+    nl, nr = lk.numel(), rk.numel()
+    world = comm.size if comm else 1
+    if capacity is None:
+        capacity = max(nl + (nr if kind == JOIN_FULL_OUTER else 0), 1)
+
+    def call(outs, capacity, ws):
+        cnt = C.c_int64(0)
+        opts = JoinOptions(odf, 0)
+        rc = lib().dj_distributed_outer_join_i64(comm.handle if comm else None, kind, _ptr(lk), _ptr(lp), nl, _ptr(rk),
+                                                 _ptr(rp), nr, *[_ptr(o) for o in outs], capacity, C.byref(cnt),
+                                                 C.byref(opts), _ptr(ws), ws.numel(), _stream())
+        return rc, cnt.value, opts
+
+    ws_bytes = None if ws is not None else lib().dj_distributed_outer_join_workspace_bytes(nl, nr, world, odf)
+    return _collective_join(comm, call, 5, capacity, ws, ws_bytes, outs, lk.device)
+
+
+def distributed_left_outer_join(comm, lk, lp, rk, rp, odf=1, capacity=None, ws=None, outs=None):
+    """SQL LEFT JOIN: every matching pair, and every left row without a match once: see distributed_outer_join."""
+    return distributed_outer_join(comm, JOIN_LEFT_OUTER, lk, lp, rk, rp, odf, capacity, ws, outs)
+
+
+def distributed_full_outer_join(comm, lk, lp, rk, rp, odf=1, capacity=None, ws=None, outs=None):
+    """SQL FULL OUTER JOIN: the left outer join plus every right row without a match once: see
+    distributed_outer_join."""
+    return distributed_outer_join(comm, JOIN_FULL_OUTER, lk, lp, rk, rp, odf, capacity, ws, outs)
 
 
 def distributed_inner_join_host(comm, h_lk, h_lp, h_rk, h_rp, h_outs, odf=1, ws=None):

@@ -256,6 +256,42 @@ int dj_distributed_left_filter_join_i64(dj_comm_t* comm, int kind,
                                         size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * dj_distributed_outer_join_i64 -- distributed left outer / full outer join (SQL LEFT JOIN and
+ * FULL OUTER JOIN; cudf::left_join / cudf::full_join) of two int64 key + int64 payload tables.
+ * Output columns are left ++ right, (left key, left payload, right key, right payload), plus one
+ * byte per row in d_out_sides saying which side of the row is present:
+ *   - every matching (left, right) pair is one row with sides = DJ_SIDE_LEFT | DJ_SIDE_RIGHT (3),
+ *     as in the inner join (duplicate keys give all pairs);
+ *   - DJ_JOIN_LEFT_OUTER: every left row whose key matches no right row appears once, with
+ *     sides = DJ_SIDE_LEFT (1);
+ *   - DJ_JOIN_FULL_OUTER: additionally every right row whose key matches no left row appears once,
+ *     with sides = DJ_SIDE_RIGHT (2).
+ * The columns of an absent side are written as 0; the sides byte is the only null marker (any int64
+ * value is a valid key).  Row order is unspecified.  An empty right table gives every left row with
+ * sides 1; an empty left table gives no rows for a left outer join and every right row with sides 2
+ * for a full outer join.  A right outer join is a left outer join with the tables swapped.
+ * Partition, exchange and the collective protocol are those of dj_distributed_inner_join_i64: comm
+ * NULL or size 1 runs the local join only; at N > 1 rank r returns the rows whose keys it owns under
+ * the murmur3 rank partition (seed 12345678); every rank must pass the same kind (otherwise every
+ * rank returns DJ_ERR_ARG before anything is exchanged); an unknown kind is DJ_ERR_ARG;
+ * DJ_ERR_WORKSPACE / opts->workspace_needed behave as for the inner join; if the output does not fit
+ * on any rank, every rank returns DJ_ERR_OVERFLOW with an exact *h_out_count, and the first
+ * out_capacity rows are written to all five columns (nothing past them).
+ */
+enum { DJ_JOIN_LEFT_OUTER = 3, DJ_JOIN_FULL_OUTER = 4 };
+/* bits of d_out_sides: which side of an output row is present */
+enum { DJ_SIDE_LEFT = 1, DJ_SIDE_RIGHT = 2 };
+size_t dj_distributed_outer_join_workspace_bytes(int64_t nleft, int64_t nright, int world,
+                                                 int over_decom_factor);
+int dj_distributed_outer_join_i64(dj_comm_t* comm, int kind,
+                                  const int64_t* d_left_key, const int64_t* d_left_payload, int64_t nleft,
+                                  const int64_t* d_right_key, const int64_t* d_right_payload, int64_t nright,
+                                  int64_t* d_out_lk, int64_t* d_out_lp, int64_t* d_out_rk, int64_t* d_out_rp,
+                                  uint8_t* d_out_sides, int64_t out_capacity, int64_t* h_out_count,
+                                  dj_join_options* opts, void* d_workspace, size_t workspace_bytes,
+                                  void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Testing: an in-process rank group.  Creates `size` communicators (ranks 0..size-1) on the
  * current device in one process; comms[r] is meant to be driven by its own host thread.  The
  * multi-rank join runs unchanged from its first control message to its overflow verdict; only
