@@ -237,7 +237,7 @@ int prepare_side(const TableInput& in, const RadixPlan& plan, PreparedSide* out,
 
 int join_prepared(const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
                   int64_t* const out[4], int64_t out_capacity, int64_t* d_out_count, bool swap,
-                  cudaStream_t stream, int kind, uint32_t* d_probe_bits, uint8_t* out_sides)
+                  cudaStream_t stream, int kind, uint32_t* d_probe_bits, uint8_t* out_sides, uint32_t* d_build_bits)
 {
   JoinBuffers jb{};
   jb.build = build.rows; jb.d_build_begin = build.d_begin; jb.d_build_end = build.d_end;
@@ -249,6 +249,7 @@ int join_prepared(const PreparedSide& build, const PreparedSide& probe, const Ra
   jb.kind         = kind;
   jb.d_probe_bits = d_probe_bits;
   jb.out_sides    = out_sides;
+  jb.d_build_bits = d_build_bits;
   return run_bucket_join(jb, swap, stream);
 }
 
@@ -278,13 +279,14 @@ int filter_join_prepared(int kind, const PreparedSide& build, const PreparedSide
 
 int outer_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
                         int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
-                        Arena& arena, cudaStream_t stream)
+                        Arena& arena, cudaStream_t stream, uint32_t* d_build_bits)
 {
   uint32_t* bits = nullptr;
   int rc         = zeroed_probe_bits(probe, arena, stream, &bits);
   if (rc) return rc;
   // the kernel writes (build row, probe row) = (right, left): swapped into left ++ right
-  return join_prepared(build, probe, plan, out, out_capacity, d_out_count, true, stream, kind, bits, out_sides);
+  return join_prepared(build, probe, plan, out, out_capacity, d_out_count, true, stream, kind, bits, out_sides,
+                       d_build_bits);
 }
 
 // Joins (bk,bp)[nb] with (pk,pp)[np]; appends matches at *d_out_count (running, device).

@@ -149,7 +149,15 @@ struct JoinBuffers {
   int kind               = 0;
   uint32_t* d_probe_bits = nullptr;
   uint8_t* out_sides     = nullptr;
+  // kJoinFullOuterMark: one bit per row POSITION of `build` (gaps between buckets included); the
+  // kernel sets the bits of the build rows it matched and never clears one
+  uint32_t* d_build_bits = nullptr;
 };
+// A join kind of the library's own, not of the ABI: one left chunk of a full outer join whose left
+// table arrives in several launches.  Its output is a left outer join's; the right rows it matched
+// are recorded in JoinBuffers::d_build_bits, and emit_unmatched_build appends the right rows no
+// launch matched once the last chunk has been joined.
+constexpr int kJoinFullOuterMark = DJ_JOIN_FULL_OUTER + 1;
 int run_bucket_join(const JoinBuffers& jb, bool swap_output_sides, cudaStream_t stream);
 // Appends the rows of segments [d_seg_begin[i], d_seg_end[i]) (each at most max_seg_rows long) to
 // (out_key, out_pay) at the running count *d_out_count, in no particular order.  With out_sides set
@@ -158,6 +166,12 @@ int append_segment_rows(const Row* rows, const int64_t* d_seg_begin, const int64
                         int64_t max_seg_rows, int64_t* out_key, int64_t* out_pay, int64_t out_capacity,
                         int64_t* d_out_count, cudaStream_t stream, int64_t* null_key = nullptr,
                         int64_t* null_pay = nullptr, uint8_t* out_sides = nullptr, uint8_t sides = 0);
+
+// Appends every row of buckets [d_begin[b], d_end[b]) of `rows` whose bit in d_build_bits (indexed by
+// row position) is clear as (0, 0, key, payload) with sides DJ_SIDE_RIGHT, at the running count.
+int emit_unmatched_build(const Row* rows, const int64_t* d_begin, const int64_t* d_end, int nbuckets,
+                         const uint32_t* d_build_bits, int64_t* const out[4], uint8_t* out_sides,
+                         int64_t out_capacity, int64_t* d_out_count, cudaStream_t stream);
 
 // Radix plan for a local join with `nbuild` build rows.
 struct RadixPlan {
@@ -220,7 +234,7 @@ int prepare_side(const TableInput& in, const RadixPlan& plan, PreparedSide* out,
 int join_prepared(const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
                   int64_t* const out[4], int64_t out_capacity, int64_t* d_out_count, bool swap,
                   cudaStream_t stream, int kind = 0, uint32_t* d_probe_bits = nullptr,
-                  uint8_t* out_sides = nullptr);
+                  uint8_t* out_sides = nullptr, uint32_t* d_build_bits = nullptr);
 // Semi / anti join of the probe side's rows against the build side's keys: zeroes the probe-row
 // bit array (taken from `arena`) and runs the join kernel of that kind; out = (key, payload).
 int filter_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
@@ -228,10 +242,11 @@ int filter_join_prepared(int kind, const PreparedSide& build, const PreparedSide
                          Arena& arena, cudaStream_t stream);
 // Left / full outer join of the probe (left) side against the build (right) side: zeroes the
 // probe-row bit array (taken from `arena`) and runs the join kernel of that kind.  out = (left key,
-// left payload, right key, right payload), out_sides = DJ_SIDE_* bits of every row.
+// left payload, right key, right payload), out_sides = DJ_SIDE_* bits of every row.  kind
+// kJoinFullOuterMark also takes d_build_bits, (build.cap_rows + 31) / 32 words zeroed once by the caller.
 int outer_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
                         int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
-                        Arena& arena, cudaStream_t stream);
+                        Arena& arena, cudaStream_t stream, uint32_t* d_build_bits = nullptr);
 int local_join(const int64_t* bk, const int64_t* bp, int64_t nb, const int64_t* pk,
                const int64_t* pp, int64_t np, int64_t* const out[4], int64_t out_capacity,
                int64_t* d_out_count, bool swap, Arena& arena, cudaStream_t stream);

@@ -43,6 +43,14 @@
 // rows without a match, and they are emitted with an absent probe side.  Output tiles of these kinds
 // carry a sides byte next to the four columns (bit 0: probe / left row present, bit 1: build / right
 // row present); absent columns are written as 0.
+//
+// A full outer join whose left table arrives in several launches (the streamed host entry joins it
+// chunk by chunk) cannot use that per-job verdict: a right row is unmatched only if no chunk matched
+// it.  KIND = kJoinFullOuterMark is a left outer join that keeps the same shared-memory bits and, at
+// the end of a job, ORs them into one global bit per row position of the build side (d.build_bits,
+// zeroed once per call).  After the last chunk emit_unmatched_build_kernel appends the build rows
+// whose bit is still clear.
+#include <algorithm>
 #include <cstdlib>
 #include <type_traits>
 
@@ -84,15 +92,21 @@ struct JoinDev {
   unsigned long long* out_count;
   uint32_t* probe_bits;  // semi / anti / outer: one bit per row of `probe` (multi-job buckets only)
   uint8_t* out_sides;    // outer joins: DJ_SIDE_* bits of every output row
+  uint32_t* build_bits;  // kMark: one bit per row position of `build`, set for matched rows
 };
 
 constexpr int kInner = 0, kSemi = DJ_JOIN_LEFT_SEMI, kAnti = DJ_JOIN_LEFT_ANTI;
-constexpr int kLeftOuter = DJ_JOIN_LEFT_OUTER, kFullOuter = DJ_JOIN_FULL_OUTER;
+constexpr int kLeftOuter = DJ_JOIN_LEFT_OUTER, kFullOuter = DJ_JOIN_FULL_OUTER, kMark = kJoinFullOuterMark;
 // sides byte of an outer join's output row, in the kernel's (build, probe) terms: the probe side is
 // the left table, the build side the right one
 constexpr uint8_t kSideProbe = DJ_SIDE_LEFT, kSideBuild = DJ_SIDE_RIGHT;
 
-__host__ __device__ constexpr bool is_outer(int kind) { return kind == kLeftOuter || kind == kFullOuter; }
+__host__ __device__ constexpr bool is_outer(int kind)
+{
+  return kind == kLeftOuter || kind == kFullOuter || kind == kMark;
+}
+// kinds that keep a "matched" bit per staged build row
+__host__ __device__ constexpr bool marks_build(int kind) { return kind == kFullOuter || kind == kMark; }
 
 template <class C>
 struct __align__(128) JoinSmem {
@@ -108,8 +122,8 @@ struct __align__(128) JoinSmem {
   int scnt[kOutTiles];
 };
 
-// Outer joins: the output tiles' sides bytes, and (full outer) one "matched" bit per staged build
-// row of each of the two tables.
+// Outer joins: the output tiles' sides bytes, and (full outer, mark) one "matched" bit per staged
+// build row of each of the two tables.
 template <class C>
 struct __align__(128) OuterJoinSmem : JoinSmem<C> {
   uint8_t ssides[kOutTiles][C::kOutRows];
@@ -131,7 +145,7 @@ __device__ __forceinline__ void consumer_sync()
 template <int KIND, class S>
 __device__ __forceinline__ int next_valid_bucket(const S& s, int lb, int nd)
 {
-  if constexpr (KIND == kAnti || KIND == kLeftOuter) {
+  if constexpr (KIND == kAnti || KIND == kLeftOuter || KIND == kMark) {
     while (lb < nd && s.dpe[lb] == s.dpb[lb]) lb++;
   } else if constexpr (KIND == kFullOuter) {
     while (lb < nd && s.dbe[lb] == s.dbb[lb] && s.dpe[lb] == s.dpb[lb]) lb++;
@@ -217,7 +231,7 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int i = tid; i < 2 * C::kSlots; i += C::kThreads) (&s.slots[0][0])[i] = 0;
-  if constexpr (KIND == kFullOuter)
+  if constexpr (marks_build(KIND))
     for (int i = tid; i < 2 * (C::kBuildChunk / 32); i += C::kThreads) (&s.bmatch[0][0])[i] = 0;
   __syncthreads();
 
@@ -355,7 +369,7 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
                 if (found) {
                   matched = true;
                   bpay    = brow[idx].pay;
-                  if constexpr (KIND == kFullOuter) {
+                  if constexpr (marks_build(KIND)) {
                     uint32_t* w      = &s.bmatch[bs][idx >> 5];
                     const uint32_t b = 1u << (idx & 31);
                     if (!(*w & b)) atomicOr(w, b);
@@ -511,6 +525,27 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
             }
             consumer_sync<kConsumers>();
           }
+          if constexpr (KIND == kMark) {
+            // This job's matched bits move to the global array at the job's row position c0.  Thread i
+            // owns word i of bmatch[bs] from this barrier on: the job's atomicOrs all precede the
+            // barrier above, nothing sets a bit of bmatch[bs] again before the probe phase of job
+            // u + 2, and every thread reaches that phase only through job u + 1's two barriers, which
+            // this thread passes after the flush.  So a plain read and a plain store of 0 are
+            // ordered, no second barrier is needed, and the build phase does not clear bmatch for
+            // this kind.  Buckets start at any row, so a word straddles two global words, which
+            // neighbouring jobs (of this or another CTA) may share: atomicOr.
+            if (tid < C::kBuildChunk / 32) {
+              const uint32_t w = s.bmatch[bs][tid];
+              if (w) {
+                s.bmatch[bs][tid] = 0;
+                const int64_t at  = c0 + 32 * tid;
+                uint32_t* g       = d.build_bits + (at >> 5);
+                const int sh      = (int)(at & 31);
+                atomicOr(g, w << sh);
+                if (sh && (w >> (32 - sh))) atomicOr(g + 1, w >> (32 - sh));
+              }
+            }
+          }
           if (lane == 0) mbar_arrive(&s.empty_build[bs]);
           if (pend_n) {
             // copy out the tile whose atomicAdd was issued one build job ago (latency hidden);
@@ -590,6 +625,7 @@ int launch_join_kind(const JoinDev& d, int kind, int ctas_per_sm, cudaStream_t s
          : kind == kAnti      ? launch_join<C, kAnti>(d, ctas_per_sm, stream)
          : kind == kLeftOuter ? launch_join<C, kLeftOuter>(d, ctas_per_sm, stream)
          : kind == kFullOuter ? launch_join<C, kFullOuter>(d, ctas_per_sm, stream)
+         : kind == kMark      ? launch_join<C, kMark>(d, ctas_per_sm, stream)
                               : launch_join<C, kInner>(d, ctas_per_sm, stream);
 }
 
@@ -622,6 +658,82 @@ __global__ void __launch_bounds__(256) append_rows_kernel(const Row* rows, const
           out_sides[g] = sides;
         }
       }
+    }
+  }
+}
+
+// After the last chunk of a streamed full outer join: every build (right) row whose bit in `bits` is
+// clear was matched by no left row of any chunk, and is appended as (0, 0, key, payload) with sides
+// kSideBuild.  The build side is walked bucket by bucket (the gaps between buckets hold stale rows);
+// a block takes a bucket in tiles of kEmitTile rows, and reserves a tile's output rows with ONE
+// global atomicAdd: the warps' ballots are scanned in shared memory.
+constexpr int kEmitThreads = 256, kEmitPerThread = 4, kEmitTile = kEmitThreads * kEmitPerThread;
+
+__global__ void __launch_bounds__(kEmitThreads) emit_unmatched_build_kernel(
+  const Row* rows, const int64_t* bbeg, const int64_t* bend, int nbuckets, const uint32_t* bits, int64_t* null_key,
+  int64_t* null_pay, int64_t* out_key, int64_t* out_pay, uint8_t* out_sides, int64_t out_capacity,
+  unsigned long long* out_count)
+{
+  constexpr int kRuns = kEmitTile / 32;  // (warp, step) runs of 32 rows in a tile
+  __shared__ unsigned long long run_base[kRuns];
+  __shared__ int run_cnt[kRuns];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int b = blockIdx.x; b < nbuckets; b += gridDim.x) {
+    const int64_t b0 = bbeg[b], b1 = bend[b];
+    for (int64_t t0 = b0; t0 < b1; t0 += kEmitTile) {
+      int4 row[kEmitPerThread];
+      unsigned lone[kEmitPerThread];
+#pragma unroll
+      for (int j = 0; j < kEmitPerThread; j++) {
+        const int64_t r = t0 + j * kEmitThreads + threadIdx.x;
+        bool mine       = false;
+        row[j]          = make_int4(0, 0, 0, 0);
+        if (r < b1 && !((bits[r >> 5] >> (r & 31)) & 1u)) {
+          mine   = true;
+          row[j] = __ldg(reinterpret_cast<const int4*>(rows + r));  // one 16-byte load per row
+        }
+        lone[j] = __ballot_sync(0xffffffffu, mine);
+        if (lane == 0) run_cnt[j * (kEmitThreads / 32) + warp] = __popc(lone[j]);
+      }
+      __syncthreads();
+      if (warp == 0) {
+        // exclusive scan of the kRuns counts (kRuns / 32 per lane), one reservation for the tile
+        int c[kRuns / 32], sum = 0;
+#pragma unroll
+        for (int i = 0; i < kRuns / 32; i++) {
+          c[i] = run_cnt[lane * (kRuns / 32) + i];
+          sum += c[i];
+        }
+        int incl = sum;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const int v = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += v;
+        }
+        const int total      = __shfl_sync(0xffffffffu, incl, 31);
+        unsigned long long g = 0;
+        if (lane == 0 && total) g = atomicAdd(out_count, (unsigned long long)total);
+        g = __shfl_sync(0xffffffffu, g, 0) + (unsigned long long)(incl - sum);
+#pragma unroll
+        for (int i = 0; i < kRuns / 32; i++) {
+          run_base[lane * (kRuns / 32) + i] = g;
+          g += c[i];
+        }
+      }
+      __syncthreads();
+#pragma unroll
+      for (int j = 0; j < kEmitPerThread; j++) {
+        if (!((lone[j] >> lane) & 1u)) continue;
+        const int64_t g = (int64_t)run_base[j * (kEmitThreads / 32) + warp] + __popc(lone[j] & lanemask_lt());
+        if (g < out_capacity) {
+          null_key[g]  = 0;
+          null_pay[g]  = 0;
+          out_key[g]   = (int64_t)(((uint64_t)(uint32_t)row[j].y << 32) | (uint32_t)row[j].x);
+          out_pay[g]   = (int64_t)(((uint64_t)(uint32_t)row[j].w << 32) | (uint32_t)row[j].z);
+          out_sides[g] = kSideBuild;
+        }
+      }
+      // the next tile writes run_base only past its first barrier, i.e. after every thread's reads above
     }
   }
 }
@@ -660,6 +772,7 @@ int run_bucket_join(const JoinBuffers& jb, bool swap_output_sides, cudaStream_t 
   d.out_count    = (unsigned long long*)jb.d_out_count;
   d.probe_bits   = jb.d_probe_bits;
   d.out_sides    = jb.out_sides;
+  d.build_bits   = jb.d_build_bits;
   return join_shape() == 1 ? launch_join_kind<CfgB>(d, jb.kind, 2, stream)
                            : launch_join_kind<CfgA>(d, jb.kind, 1, stream);
 }
@@ -676,6 +789,22 @@ int append_segment_rows(const Row* rows, const int64_t* d_seg_begin, const int64
     ProfScope prof(DJ_PROF_OTHER, stream);
     append_rows_kernel<<<grid, 256, 0, stream>>>(rows, d_seg_begin, d_seg_end, out_key, out_pay, null_key, null_pay,
                                                  out_sides, sides, out_capacity, (unsigned long long*)d_out_count);
+  }
+  DJ_LAUNCH_CHECK();
+  return DJ_OK;
+}
+
+int emit_unmatched_build(const Row* rows, const int64_t* d_begin, const int64_t* d_end, int nbuckets,
+                         const uint32_t* d_build_bits, int64_t* const out[4], uint8_t* out_sides,
+                         int64_t out_capacity, int64_t* d_out_count, cudaStream_t stream)
+{
+  if (nbuckets <= 0) return DJ_OK;
+  const int grid = std::min(nbuckets, sm_count() * 8);
+  {
+    ProfScope prof(DJ_PROF_OTHER, stream);
+    emit_unmatched_build_kernel<<<grid, kEmitThreads, 0, stream>>>(rows, d_begin, d_end, nbuckets, d_build_bits, out[0],
+                                                                   out[1], out[2], out[3], out_sides, out_capacity,
+                                                                   (unsigned long long*)d_out_count);
   }
   DJ_LAUNCH_CHECK();
   return DJ_OK;

@@ -82,6 +82,8 @@ ABI_SYMBOLS = [
     "dj_distributed_inner_join_i64_host", "dj_comm_create_local_group", "dj_testing_radix_repairs",
     "dj_distributed_left_filter_join_workspace_bytes", "dj_distributed_left_filter_join_i64",
     "dj_distributed_outer_join_workspace_bytes", "dj_distributed_outer_join_i64",
+    "dj_distributed_left_filter_join_host_workspace_bytes", "dj_distributed_left_filter_join_i64_host",
+    "dj_distributed_outer_join_host_workspace_bytes", "dj_distributed_outer_join_i64_host",
 ]
 
 _lib = None
@@ -142,6 +144,11 @@ def lib() -> C.CDLL:
     L.dj_distributed_outer_join_workspace_bytes.argtypes = [i64, i64, C.c_int, C.c_int]
     L.dj_distributed_outer_join_i64.argtypes = [vp, C.c_int, vp, vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, i64,
                                                 C.POINTER(i64), C.POINTER(JoinOptions), vp, sz, vp]
+    for fn in (L.dj_distributed_left_filter_join_host_workspace_bytes, L.dj_distributed_outer_join_host_workspace_bytes):
+        fn.restype = sz
+        fn.argtypes = [i64, i64, i64, C.c_int, C.c_int]
+    L.dj_distributed_left_filter_join_i64_host.argtypes = L.dj_distributed_left_filter_join_i64.argtypes
+    L.dj_distributed_outer_join_i64_host.argtypes = L.dj_distributed_outer_join_i64.argtypes
     L.dj_comm_create_local_group.argtypes = [C.c_int, C.POINTER(vp)]
     L.dj_testing_radix_repairs.argtypes = [C.POINTER(i64)]
     _lib = L
@@ -499,6 +506,29 @@ def distributed_full_outer_join(comm, lk, lp, rk, rp, odf=1, capacity=None, ws=N
     return distributed_outer_join(comm, JOIN_FULL_OUTER, lk, lp, rk, rp, odf, capacity, ws, outs)
 
 
+def _host_join(comm, name, call, ws, ws_bytes):
+    """The host entries' collective grow-and-retry.  `call(ws)` runs one join and returns (rc, n_out,
+    options).  A workspace that is too small on any rank is grown and the call retried on every rank,
+    as in _collective_join; the host outputs belong to the caller, so an overflow raises (on every
+    rank)."""
+    world = comm.size if comm else 1
+    if ws is None:
+        ws = workspace(ws_bytes())
+    while True:
+        rc, n, opts = call(ws)
+        _check(rc, allow=(ERR_WORKSPACE,) if world > 1 else ())
+        if rc == 0:
+            return n, opts
+        comm.release_workspace()
+        need = int(opts.workspace_needed)
+        # collective: a retry that no rank's workspace grows for would fail the same way forever
+        if not any(comm.allgather_i64([1 if need > ws.numel() else 0])):
+            raise DjError(f"{name}: no rank needs a larger workspace, yet rank {comm.rank} "
+                          f"got DJ_ERR_WORKSPACE: {lib().dj_last_error().decode()}")
+        ws = workspace(max(ws.numel(), need + need // 8))
+        comm.barrier()
+
+
 def distributed_inner_join_host(comm, h_lk, h_lp, h_rk, h_rp, h_outs, odf=1, ws=None):
     """End-to-end entry: HOST (pinned) inputs and outputs, copies inside the call.  A workspace that
     is too small on any rank is grown and the call retried on every rank, as in distributed_inner_join;
@@ -506,23 +536,57 @@ def distributed_inner_join_host(comm, h_lk, h_lp, h_rk, h_rp, h_outs, odf=1, ws=
     nl, nr = h_lk.numel(), h_rk.numel()
     capacity = h_outs[0].numel()
     world = comm.size if comm else 1
-    if ws is None:
-        ws = workspace(lib().dj_distributed_inner_join_host_workspace_bytes(nl, nr, capacity, world, odf))
-    while True:
+
+    def call(ws):
         cnt = C.c_int64(0)
         opts = JoinOptions(odf, 0, 0, 0, 0, 0)
-        rc = _check(lib().dj_distributed_inner_join_i64_host(comm.handle if comm else None, _ptr(h_lk), _ptr(h_lp),
-                                                             nl, _ptr(h_rk), _ptr(h_rp), nr,
-                                                             *[_ptr(o) for o in h_outs], capacity, C.byref(cnt),
-                                                             C.byref(opts), _ptr(ws), ws.numel(), _stream()),
-                    allow=(ERR_WORKSPACE,) if world > 1 else ())
-        if rc == 0:
-            return cnt.value, opts
-        comm.release_workspace()
-        need = int(opts.workspace_needed)
-        # collective: a retry that no rank's workspace grows for would fail the same way forever
-        if not any(comm.allgather_i64([1 if need > ws.numel() else 0])):
-            raise DjError(f"distributed_inner_join_host: no rank needs a larger workspace, yet rank {comm.rank} "
-                          f"got DJ_ERR_WORKSPACE: {lib().dj_last_error().decode()}")
-        ws = workspace(max(ws.numel(), need + need // 8))
-        comm.barrier()
+        rc = lib().dj_distributed_inner_join_i64_host(comm.handle if comm else None, _ptr(h_lk), _ptr(h_lp), nl,
+                                                      _ptr(h_rk), _ptr(h_rp), nr, *[_ptr(o) for o in h_outs],
+                                                      capacity, C.byref(cnt), C.byref(opts), _ptr(ws), ws.numel(),
+                                                      _stream())
+        return rc, cnt.value, opts
+
+    return _host_join(comm, "distributed_inner_join_host", call, ws,
+                      lambda: lib().dj_distributed_inner_join_host_workspace_bytes(nl, nr, capacity, world, odf))
+
+
+def distributed_left_filter_join_host(comm, kind, h_lk, h_lp, h_rk, h_outs, odf=1, ws=None):
+    """Left semi / left anti join of HOST (pinned) tables into the two host columns `h_outs`, whose
+    length is the capacity: dj_distributed_left_filter_join_i64_host.  Returns (count, options); the
+    retry and overflow rules are distributed_inner_join_host's."""
+    nl, nr = h_lk.numel(), h_rk.numel()
+    capacity = h_outs[0].numel()
+    world = comm.size if comm else 1
+
+    def call(ws):
+        cnt = C.c_int64(0)
+        opts = JoinOptions(odf, 0)
+        rc = lib().dj_distributed_left_filter_join_i64_host(comm.handle if comm else None, kind, _ptr(h_lk),
+                                                            _ptr(h_lp), nl, _ptr(h_rk), nr, _ptr(h_outs[0]),
+                                                            _ptr(h_outs[1]), capacity, C.byref(cnt), C.byref(opts),
+                                                            _ptr(ws), ws.numel(), _stream())
+        return rc, cnt.value, opts
+
+    return _host_join(comm, "distributed_left_filter_join_host", call, ws,
+                      lambda: lib().dj_distributed_left_filter_join_host_workspace_bytes(nl, nr, capacity, world, odf))
+
+
+def distributed_outer_join_host(comm, kind, h_lk, h_lp, h_rk, h_rp, h_outs, odf=1, ws=None):
+    """Left outer / full outer join of HOST (pinned) tables into `h_outs`, four int64 host columns and
+    a uint8 sides column whose length is the capacity: dj_distributed_outer_join_i64_host.  Returns
+    (count, options); the retry and overflow rules are distributed_inner_join_host's."""
+    nl, nr = h_lk.numel(), h_rk.numel()
+    capacity = h_outs[0].numel()
+    world = comm.size if comm else 1
+
+    def call(ws):
+        cnt = C.c_int64(0)
+        opts = JoinOptions(odf, 0)
+        rc = lib().dj_distributed_outer_join_i64_host(comm.handle if comm else None, kind, _ptr(h_lk), _ptr(h_lp), nl,
+                                                      _ptr(h_rk), _ptr(h_rp), nr, *[_ptr(o) for o in h_outs],
+                                                      capacity, C.byref(cnt), C.byref(opts), _ptr(ws), ws.numel(),
+                                                      _stream())
+        return rc, cnt.value, opts
+
+    return _host_join(comm, "distributed_outer_join_host", call, ws,
+                      lambda: lib().dj_distributed_outer_join_host_workspace_bytes(nl, nr, capacity, world, odf))

@@ -292,6 +292,50 @@ int dj_distributed_outer_join_i64(dj_comm_t* comm, int kind,
                                   void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * dj_distributed_left_filter_join_i64_host / dj_distributed_outer_join_i64_host -- the semi, anti,
+ * left outer and full outer joins with HOST input and output columns (pinned recommended).  They
+ * replace what a caller of cudf::left_semi_join / left_anti_join / left_join / full_join with tables
+ * in host memory does around the call: copy both tables up, join, copy the result down, three serial
+ * phases.  Arguments are those of dj_distributed_left_filter_join_i64 / dj_distributed_outer_join_i64
+ * with h_ pointers, and so are the results: the same row classes, sides bytes, zeros for an absent
+ * side, unspecified row order, DJ_ERR_ARG for an unknown kind.
+ *   - comm NULL or size 1: the call is organised around the PCIe link like
+ *     dj_distributed_inner_join_i64_host.  The right table goes up once and is the build side; the
+ *     left table goes up in double-buffered chunks; every chunk is joined as it lands and its rows go
+ *     down while the next chunk comes up.  A full outer join's unmatched right rows are known only
+ *     after the last chunk and go down last.
+ *   - N > 1: the columns are staged at the front of the workspace, the device entry of the same kind
+ *     runs on the rest, and the result is copied down (collective, as the device entry).
+ * Overflow: DJ_ERR_OVERFLOW with the exact *h_out_count; the first out_capacity rows are written
+ * and nothing past them, in any of the 2 or 5 host columns.  An empty table gives what the device
+ * entries give (every left row for anti / outer joins against an empty right table, every right row
+ * for a full outer join of an empty left table), copied from host column to host column.
+ * Workspace: *_host_workspace_bytes is what the call needs; with less it returns DJ_ERR_WORKSPACE and
+ * opts->workspace_needed is the whole workspace, staged columns included.  The outer query is sized
+ * for a full outer join.  The calls synchronise the stream before they return.
+ */
+size_t dj_distributed_left_filter_join_host_workspace_bytes(int64_t nleft, int64_t nright,
+                                                            int64_t out_capacity, int world,
+                                                            int over_decom_factor);
+int dj_distributed_left_filter_join_i64_host(dj_comm_t* comm, int kind,
+                                             const int64_t* h_left_key, const int64_t* h_left_payload,
+                                             int64_t nleft, const int64_t* h_right_key, int64_t nright,
+                                             int64_t* h_out_key, int64_t* h_out_payload,
+                                             int64_t out_capacity, int64_t* h_out_count,
+                                             dj_join_options* opts, void* d_workspace,
+                                             size_t workspace_bytes, void* stream);
+size_t dj_distributed_outer_join_host_workspace_bytes(int64_t nleft, int64_t nright,
+                                                      int64_t out_capacity, int world,
+                                                      int over_decom_factor);
+int dj_distributed_outer_join_i64_host(dj_comm_t* comm, int kind,
+                                       const int64_t* h_left_key, const int64_t* h_left_payload, int64_t nleft,
+                                       const int64_t* h_right_key, const int64_t* h_right_payload, int64_t nright,
+                                       int64_t* h_out_lk, int64_t* h_out_lp, int64_t* h_out_rk, int64_t* h_out_rp,
+                                       uint8_t* h_out_sides, int64_t out_capacity, int64_t* h_out_count,
+                                       dj_join_options* opts, void* d_workspace, size_t workspace_bytes,
+                                       void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Testing: an in-process rank group.  Creates `size` communicators (ranks 0..size-1) on the
  * current device in one process; comms[r] is meant to be driven by its own host thread.  The
  * multi-rank join runs unchanged from its first control message to its overflow verdict; only
