@@ -2,24 +2,25 @@
 //
 // Replaces cudf::inner_join as called by local_join_helper (src/distributed_join.cpp:71-83).
 // Both tables arrive radix-partitioned (partition.cu, mode 1) into buckets whose build side
-// fits one CTA's shared-memory table.  One persistent CTA per SM (31 consumer warps + 1
-// producer warp) walks a contiguous range of buckets:
+// fits one group's shared-memory table.  One persistent CTA per SM walks a contiguous range of
+// buckets with two independent consumer groups of 15 consumer warps + 1 producer warp each; group g
+// takes the buckets of even (g = 0) or odd (g = 1) ordinal in the walk, on its own buffers, mbarriers
+// and named barrier, so that while one group waits at a barrier or for rows, the other probes:
 //
-//   producer warp   one elected lane streams every bucket's rows HBM -> shared memory with TMA
-//                   bulk copies (cp.async.bulk + mbarrier complete_tx): one build-chunk stage
-//                   and a ring of probe-chunk stages, refilled as soon as consumers release them,
-//                   so global-memory latency never sits on the consumers' critical path;
+//   producer warp   one elected lane streams the group's buckets HBM -> shared memory with TMA
+//                   bulk copies (cp.async.bulk + mbarrier complete_tx): one build-chunk stage,
+//                   refilled as soon as the group's job releases it, and a ring of probe-chunk
+//                   stages, refilled as soon as consumers release them;
 //   consumer warps  1. insert the staged build rows (16-byte (key, payload) rows, one TMA copy per
 //                      chunk) into a linear-probing table of 32-bit (fingerprint, row) slots claimed
 //                      with atomicCAS -- the staged rows are the row store, no key value is reserved
-//                      as "empty"; two tables ping-pong so the next one is cleared off the critical
-//                      path,
+//                      as "empty"; the table is cleared at the end of each job,
 //                   2. probe one staged row per lane; matches are compacted with __ballot_sync /
 //                      popc into a shared-memory output tile,
-//                   3. flush full output tiles with ONE global atomicAdd per tile and coalesced
-//                      stores; the atomic's round trip is hidden behind the next round of probing
-//                      (three tiles rotate), and batch results land in one output so no
-//                      cudf::concatenate is needed afterwards.
+//                   3. reserve the tile's rows with ONE global atomicAdd at the end of a job, and
+//                      copy it out with coalesced stores after the next job's first barrier, so the
+//                      atomic's round trip overlaps the table clear; batch results land in one
+//                      output so no cudf::concatenate is needed afterwards.
 // Multimap semantics: probing continues past a hit until an empty slot.  Build buckets larger
 // than one chunk (skew / duplicates) are processed chunk by chunk, re-streaming the probe side.
 //
@@ -30,7 +31,7 @@
 // jobs, a row's verdict is kept across the jobs in one bit per prepared probe row (d.probe_bits,
 // zeroed before the launch): semi emits a row when its atomicOr finds the bit clear, anti sets
 // bits in every job but the last and emits, in the last, the rows with neither a bit nor a match.
-// The jobs of a bucket run in order in one CTA, and the consumer barrier between two jobs orders
+// The jobs of a bucket run in order in one consumer group, and its barriers between two jobs order
 // the bit updates.  An anti join also runs one (empty) build job for a bucket whose build side is
 // empty, so that its probe rows are all emitted.
 //
@@ -61,24 +62,27 @@ namespace dj {
 
 namespace {
 
-// Compile-time shape of one CTA.  Two shapes are built: A = one 1024-thread CTA per SM for
-// ~1.5K-row buckets, B = two 512-thread CTAs per SM for ~0.75K-row buckets.
-template <int THREADS, int SLOTS, int BUILD_CHUNK, int TARGET_ROWS, int PROBE_STAGES, int OUT_ROWS>
+// Compile-time shape of one CTA.  A CTA is GROUPS independent groups of 512 threads (15 consumer
+// warps + 1 producer warp), each running the whole per-bucket pipeline on its own buffers, barriers
+// and share of the CTA's buckets.  Two shapes are built: A = one CTA per SM of two groups for ~1.5K-row
+// buckets, B = two one-group CTAs per SM for ~0.75K-row buckets.
+template <int GROUPS, int SLOTS, int BUILD_CHUNK, int TARGET_ROWS, int PROBE_STAGES, int OUT_ROWS>
 struct JoinCfg {
-  static constexpr int kThreads     = THREADS;
-  static constexpr int kConsumers   = THREADS - 32;
-  static constexpr int kConsWarps   = kConsumers / 32;
-  static constexpr int kSlots       = SLOTS;        // 32-bit slots per table (power of 2)
-  static constexpr int kBuildChunk  = BUILD_CHUNK;  // max build rows per table (<= 2048)
-  static constexpr int kTargetRows  = TARGET_ROWS;  // planned average build rows per bucket
-  static constexpr int kProbeChunk  = kConsumers;   // one probe row per consumer thread and round
-  static constexpr int kProbeStages = PROBE_STAGES;
-  static constexpr int kOutRows     = OUT_ROWS;     // rows per output tile
+  static constexpr int kGroups       = GROUPS;
+  static constexpr int kGroupThreads = 512;
+  static constexpr int kThreads      = GROUPS * kGroupThreads;
+  static constexpr int kConsumers    = kGroupThreads - 32;  // per group
+  static constexpr int kConsWarps    = kConsumers / 32;
+  static constexpr int kSlots        = SLOTS;        // 32-bit slots per table (power of 2)
+  static constexpr int kBuildChunk   = BUILD_CHUNK;  // max build rows per table (<= 2048)
+  static constexpr int kTargetRows   = TARGET_ROWS;  // planned average build rows per bucket
+  static constexpr int kProbeChunk   = kConsumers;   // one probe row per consumer thread and round
+  static constexpr int kProbeStages  = PROBE_STAGES;
+  static constexpr int kOutRows      = OUT_ROWS;     // rows per output tile
 };
-using CfgA = JoinCfg<1024, 8192, 1792, 1536, 2, 576>;
-using CfgB = JoinCfg<512, 4096, 1024, 768, 2, 256>;
+using CfgA = JoinCfg<2, 8192, 1792, 1536, 2, 1024>;
+using CfgB = JoinCfg<1, 4096, 1024, 768, 2, 512>;
 
-constexpr int kOutTiles    = 3;    // filling / atomicAdd in flight / draining
 constexpr int kDescBuckets = 128;  // bucket descriptors cached per refill
 
 struct JoinDev {
@@ -108,35 +112,46 @@ __host__ __device__ constexpr bool is_outer(int kind)
 // kinds that keep a "matched" bit per staged build row
 __host__ __device__ constexpr bool marks_build(int kind) { return kind == kFullOuter || kind == kMark; }
 
+// One consumer group's buffers: its table, build stage, probe ring and output tile.
 template <class C>
-struct __align__(128) JoinSmem {
-  uint32_t slots[2][C::kSlots];
-  Row brow[2][C::kBuildChunk];
+struct __align__(128) JoinGroup {
+  uint32_t slots[C::kSlots];
+  Row brow[C::kBuildChunk];
   Row prow[C::kProbeStages][C::kProbeChunk];
-  int64_t sout[kOutTiles][4][C::kOutRows];
-  int64_t dbb[kDescBuckets], dbe[kDescBuckets];  // cached bucket ranges, build side
-  int64_t dpb[kDescBuckets], dpe[kDescBuckets];  // probe side
-  unsigned long long full_build[2], empty_build[2];
+  int64_t sout[4][C::kOutRows];
+  unsigned long long full_build, empty_build;
   unsigned long long full_probe[C::kProbeStages], empty_probe[C::kProbeStages];
-  unsigned long long sbase[kOutTiles];
-  int scnt[kOutTiles];
+  unsigned long long sbase;  // the tile's output position, reserved at the end of a job
+  int scnt;                  // rows in the tile
 };
 
-// Outer joins: the output tiles' sides bytes, and (full outer, mark) one "matched" bit per staged
-// build row of each of the two tables.
+// Outer joins: the output tile's sides bytes, and (full outer, mark) one "matched" bit per staged
+// build row.
 template <class C>
-struct __align__(128) OuterJoinSmem : JoinSmem<C> {
-  uint8_t ssides[kOutTiles][C::kOutRows];
-  uint32_t bmatch[2][C::kBuildChunk / 32];
+struct __align__(128) OuterJoinGroup : JoinGroup<C> {
+  uint8_t ssides[C::kOutRows];
+  uint32_t bmatch[C::kBuildChunk / 32];
 };
 
 template <class C, int KIND>
-using JoinSmemOf = std::conditional_t<is_outer(KIND), OuterJoinSmem<C>, JoinSmem<C>>;
+using JoinGroupOf = std::conditional_t<is_outer(KIND), OuterJoinGroup<C>, JoinGroup<C>>;
 
+template <class C, int KIND>
+struct __align__(128) JoinSmem {
+  JoinGroupOf<C, KIND> grp[C::kGroups];
+  int64_t dbb[kDescBuckets], dbe[kDescBuckets];  // cached bucket ranges, build side
+  int64_t dpb[kDescBuckets], dpe[kDescBuckets];  // probe side
+};
+
+// Named barrier 1 + g of group g's consumer warps (barrier 0 is __syncthreads).  Immediate ids, so
+// that the kernel reserves three barriers and not all sixteen.
 template <int N>
-__device__ __forceinline__ void consumer_sync()
+__device__ __forceinline__ void group_sync(int g)
 {
-  asm volatile("bar.sync 1, %0;" ::"n"(N) : "memory");
+  if (g == 0)
+    asm volatile("bar.sync 1, %0;" ::"n"(N) : "memory");
+  else
+    asm volatile("bar.sync 2, %0;" ::"n"(N) : "memory");
 }
 
 // Build jobs of the cached descriptor block: (bucket, build chunk) pairs whose bucket is
@@ -155,14 +170,24 @@ __device__ __forceinline__ int next_valid_bucket(const S& s, int lb, int nd)
   return lb;
 }
 
+// Group g's next bucket at or after lb: the valid buckets are numbered in the CTA's walk (`ord`
+// counts them across descriptor blocks), and group g takes those with ord % kGroups == g.
+template <class C, int KIND, class S>
+__device__ __forceinline__ int next_group_bucket(const S& s, int lb, int nd, uint32_t& ord, int g)
+{
+  for (lb = next_valid_bucket<KIND>(s, lb, nd); lb < nd; lb = next_valid_bucket<KIND>(s, lb + 1, nd))
+    if (ord++ % C::kGroups == (uint32_t)g) break;
+  return lb;
+}
+
 // Slot word: bit 31 = occupied, bits 30..11 = 20-bit key fingerprint, bits 10..0 = build row.
 __device__ __forceinline__ uint32_t slot_tag(uint32_t h) { return 0x100000u | (h >> 12); }
 
-// Outer joins: every lane with `emit` set appends the row (bk, bp, pk, pv, sides) to output tile
-// `cur`; once the tile is full, the warp reserves its own run of the output and stores the rest
+// Outer joins: every lane with `emit` set appends the row (bk, bp, pk, pv, sides) to the output
+// tile; once the tile is full, the warp reserves its own run of the output and stores the rest
 // directly.  Called by all 32 lanes of a warp.
 template <class C>
-__device__ __forceinline__ void emit_outer_row(OuterJoinSmem<C>& s, const JoinDev& d, int cur, int lane, bool emit,
+__device__ __forceinline__ void emit_outer_row(OuterJoinGroup<C>& s, const JoinDev& d, int lane, bool emit,
                                                int64_t bk, int64_t bp, int64_t pk, int64_t pv, uint8_t sides)
 {
   const unsigned m = __ballot_sync(0xffffffffu, emit);
@@ -170,18 +195,18 @@ __device__ __forceinline__ void emit_outer_row(OuterJoinSmem<C>& s, const JoinDe
   const int leader = __ffs(m) - 1;
   int obase        = 0;
   if (lane == leader) {
-    obase = atomicAdd(&s.scnt[cur], __popc(m));
-    if (obase >= C::kOutRows) atomicSub(&s.scnt[cur], __popc(m));  // a full tile stays full (see inner)
+    obase = atomicAdd(&s.scnt, __popc(m));
+    if (obase >= C::kOutRows) atomicSub(&s.scnt, __popc(m));  // a full tile stays full (see inner)
   }
   obase            = __shfl_sync(0xffffffffu, obase, leader);
   const int pos    = obase + __popc(m & lanemask_lt());
   const bool spill = emit && pos >= C::kOutRows;
   if (emit && !spill) {
-    s.sout[cur][0][pos] = bk;
-    s.sout[cur][1][pos] = bp;
-    s.sout[cur][2][pos] = pk;
-    s.sout[cur][3][pos] = pv;
-    s.ssides[cur][pos]  = sides;
+    s.sout[0][pos] = bk;
+    s.sout[1][pos] = bp;
+    s.sout[2][pos] = pk;
+    s.sout[3][pos] = pv;
+    s.ssides[pos]  = sides;
   }
   const unsigned ms = __ballot_sync(0xffffffffu, spill);
   if (ms) {
@@ -202,49 +227,64 @@ __device__ __forceinline__ void emit_outer_row(OuterJoinSmem<C>& s, const JoinDe
   }
 }
 
+// The group's consumers store the first n rows of its output tile at the reserved position sbase.
+template <class C, int KIND>
+__device__ __forceinline__ void copy_out_tile(const JoinGroupOf<C, KIND>& s, const JoinDev& d, int n, int ltid)
+{
+  constexpr int kCols = (KIND == kSemi || KIND == kAnti) ? 2 : 4;
+  const int64_t gb    = (int64_t)s.sbase;
+#pragma unroll
+  for (int c = 0; c < kCols; c++)
+    for (int i = ltid; i < n; i += C::kConsumers)
+      if (gb + i < d.out_capacity) d.out[c][gb + i] = s.sout[c][i];
+  if constexpr (is_outer(KIND))
+    for (int i = ltid; i < n; i += C::kConsumers)
+      if (gb + i < d.out_capacity) d.out_sides[gb + i] = s.ssides[i];
+}
+
 template <class C, int KIND>
 __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
 {
-  using Smem = JoinSmemOf<C, KIND>;
+  using Smem = JoinSmem<C, KIND>;
   constexpr int kConsumers = C::kConsumers;
   constexpr bool kOuter    = is_outer(KIND);
   // a bucket with probe rows but no build rows still runs one (empty) build job
   constexpr bool kEmptyJob = KIND == kAnti || kOuter;
-  constexpr int kCols      = (KIND == kSemi || KIND == kAnti) ? 2 : 4;  // output columns
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& s        = *reinterpret_cast<Smem*>(smem_raw);
   const int tid  = threadIdx.x;
   const int lane = tid & 31;
-  const int warp = tid >> 5;
-  const bool is_producer = warp == C::kConsWarps;
+  const int g    = tid / C::kGroupThreads;  // consumer group
+  const int ltid = tid % C::kGroupThreads;  // thread within the group: consumers first, then the producer warp
+  const bool is_producer = ltid >= kConsumers;
+  auto& sg = s.grp[g];
 
-  if (tid == 0) {
-    for (int i = 0; i < 2; i++) {
-      mbar_init(&s.full_build[i], 1);
-      mbar_init(&s.empty_build[i], C::kConsWarps);
-    }
+  if (ltid == 0) {
+    mbar_init(&sg.full_build, 1);
+    mbar_init(&sg.empty_build, C::kConsWarps);
     for (int i = 0; i < C::kProbeStages; i++) {
-      mbar_init(&s.full_probe[i], 1);
-      mbar_init(&s.empty_probe[i], C::kConsWarps);
+      mbar_init(&sg.full_probe[i], 1);
+      mbar_init(&sg.empty_probe[i], C::kConsWarps);
     }
-    for (int i = 0; i < kOutTiles; i++) s.scnt[i] = 0;
+    sg.scnt = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  for (int i = tid; i < 2 * C::kSlots; i += C::kThreads) (&s.slots[0][0])[i] = 0;
+  for (int i = ltid; i < C::kSlots; i += C::kGroupThreads) sg.slots[i] = 0;
   if constexpr (marks_build(KIND))
-    for (int i = tid; i < 2 * (C::kBuildChunk / 32); i += C::kThreads) (&s.bmatch[0][0])[i] = 0;
+    for (int i = ltid; i < C::kBuildChunk / 32; i += C::kGroupThreads) sg.bmatch[i] = 0;
   __syncthreads();
 
   // contiguous bucket range of this CTA
   const int lo = (int)((int64_t)d.nbuckets * blockIdx.x / gridDim.x);
   const int hi = (int)((int64_t)d.nbuckets * (blockIdx.x + 1) / gridDim.x);
 
-  uint32_t q = 0;  // probe-job ordinal (stage = q % kProbeStages)
-  uint32_t u = 0;  // build-job ordinal (stage = table = u & 1)
-  // Output tiles rotate filling -> pending (its atomicAdd is in flight during the next build
-  // job) -> draining (copied out while a third tile already fills) -> free.
-  int cur = 0, pend_tile = 0, pend_n = 0;
-  unsigned long long pend_base_reg = 0;  // thread 0 only
+  uint32_t ord = 0;  // valid-bucket ordinal in the CTA's walk (picks the group)
+  uint32_t q   = 0;  // probe-job ordinal of this group (stage = q % kProbeStages)
+  uint32_t u   = 0;  // build-job ordinal of this group (phase of its one build stage = u & 1)
+  // The output tile fills during a build job.  At the job's end ltid 0 reserves its rows with one
+  // atomicAdd, whose round trip overlaps the table clear; the group copies it out after the next
+  // job's first barrier, before that job's probe phase fills it again.
+  int pend_n = 0;
 
   for (int base = lo; base < hi; base += kDescBuckets) {
     const int nd = min(kDescBuckets, hi - base);
@@ -258,25 +298,26 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
     __syncthreads();
 
     if (is_producer) {
-      // ------------------------------------------------------------ producer (one lane)
+      // ------------------------------------------------------------ producer (one lane per group)
       if (lane == 0) {
-        for (int lb = next_valid_bucket<KIND>(s, 0, nd); lb < nd; lb = next_valid_bucket<KIND>(s, lb + 1, nd)) {
+        for (int lb = next_group_bucket<C, KIND>(s, 0, nd, ord, g); lb < nd;
+             lb     = next_group_bucket<C, KIND>(s, lb + 1, nd, ord, g)) {
           const int64_t b0 = s.dbb[lb], b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
           for (int64_t c0 = b0; c0 < b1 || (kEmptyJob && c0 == b0); c0 += C::kBuildChunk) {
             {
-              const int bs = u & 1;
-              const int n  = (int)min((int64_t)C::kBuildChunk, b1 - c0);  // 0 for an empty build job
-              mbar_wait(&s.empty_build[bs], ((u >> 1) & 1) ^ 1);
-              mbar_expect_tx(&s.full_build[bs], (uint32_t)n * 16u);
-              if (!kEmptyJob || n > 0) tma_load(s.brow[bs], d.build + c0, (uint32_t)n * 16u, &s.full_build[bs]);
+              // the stage is freed at the end of the group's previous job; refill it at once
+              const int n = (int)min((int64_t)C::kBuildChunk, b1 - c0);  // 0 for an empty build job
+              mbar_wait(&sg.empty_build, (u & 1) ^ 1);
+              mbar_expect_tx(&sg.full_build, (uint32_t)n * 16u);
+              if (!kEmptyJob || n > 0) tma_load(sg.brow, d.build + c0, (uint32_t)n * 16u, &sg.full_build);
               u++;
             }
             for (int64_t r0 = p0; r0 < p1; r0 += C::kProbeChunk) {
               const int st = q % C::kProbeStages;
               const int n  = (int)min((int64_t)C::kProbeChunk, p1 - r0);
-              mbar_wait(&s.empty_probe[st], ((q / C::kProbeStages) & 1) ^ 1);
-              mbar_expect_tx(&s.full_probe[st], (uint32_t)n * 16u);
-              tma_load(s.prow[st], d.probe + r0, (uint32_t)n * 16u, &s.full_probe[st]);
+              mbar_wait(&sg.empty_probe[st], ((q / C::kProbeStages) & 1) ^ 1);
+              mbar_expect_tx(&sg.full_probe[st], (uint32_t)n * 16u);
+              tma_load(sg.prow[st], d.probe + r0, (uint32_t)n * 16u, &sg.full_probe[st]);
               q++;
             }
           }
@@ -285,7 +326,10 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
       __syncwarp();  // reconverge before the CTA-wide barrier at the top of the loop
     } else {
       // ------------------------------------------------------------ consumers
-      for (int lb = next_valid_bucket<KIND>(s, 0, nd); lb < nd; lb = next_valid_bucket<KIND>(s, lb + 1, nd)) {
+      uint32_t* const slots = sg.slots;
+      const Row* const brow = sg.brow;
+      for (int lb = next_group_bucket<C, KIND>(s, 0, nd, ord, g); lb < nd;
+           lb     = next_group_bucket<C, KIND>(s, lb + 1, nd, ord, g)) {
         const int64_t b0 = s.dbb[lb], b1 = s.dbe[lb], p0 = s.dpb[lb], p1 = s.dpe[lb];
         // semi / anti / outer: does this bucket's build side span several jobs, and is this its last job
         const bool multi = KIND != kInner && b1 - b0 > C::kBuildChunk;
@@ -293,35 +337,32 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
           const bool last = c0 + C::kBuildChunk >= b1;
           // ---- build: fingerprint + row index into a 32-bit slot claimed with atomicCAS; the
           //      staged rows themselves are the row store (no copy)
-          const int bs = u & 1;
           const int nb = (int)min((int64_t)C::kBuildChunk, b1 - c0);
-          uint32_t* slots     = s.slots[bs];
-          const Row* brow     = s.brow[bs];
-          mbar_wait(&s.full_build[bs], (u >> 1) & 1);
-          for (int r = tid; r < nb; r += kConsumers) {
+          group_sync<kConsumers>(g);  // table cleared, previous job's tile reserved
+          if (pend_n) {
+            // copy out while the build rows land
+            copy_out_tile<C, KIND>(sg, d, pend_n, ltid);
+            if (ltid == 0) sg.scnt = 0;
+            pend_n = 0;
+          }
+          mbar_wait(&sg.full_build, u & 1);
+          for (int r = ltid; r < nb; r += kConsumers) {
             const uint32_t h = slot_hash_i64(brow[r].key);
             const uint32_t e = (slot_tag(h) << 11) | (uint32_t)r;
             uint32_t slot    = h & (C::kSlots - 1);
             while (atomicCAS(&slots[slot], 0u, e) != 0u) slot = (slot + 1) & (C::kSlots - 1);
           }
-          // the other table was last probed two build jobs ago: clear it for the next job
-          {
-            uint4* other = reinterpret_cast<uint4*>(s.slots[bs ^ 1]);
-            for (int i = tid; i < C::kSlots / 4; i += kConsumers) other[i] = make_uint4(0, 0, 0, 0);
-            if constexpr (KIND == kFullOuter)
-              for (int i = tid; i < C::kBuildChunk / 32; i += kConsumers) s.bmatch[bs ^ 1][i] = 0;
-          }
-          consumer_sync<kConsumers>();  // table complete
+          group_sync<kConsumers>(g);  // table complete
 
           // ---- probe: every warp streams its 32 rows of each staged chunk at its own pace
           for (int64_t r0 = p0; r0 < p1; r0 += C::kProbeChunk) {
             const int st = q % C::kProbeStages;
             const int np = (int)min((int64_t)C::kProbeChunk, p1 - r0);
-            mbar_wait(&s.full_probe[st], (q / C::kProbeStages) & 1);
-            bool alive = tid < np;
+            mbar_wait(&sg.full_probe[st], (q / C::kProbeStages) & 1);
+            bool alive = ltid < np;
             int64_t k = 0, v = 0;
             if (alive) {
-              const int4 pr = *reinterpret_cast<const int4*>(&s.prow[st][tid]);
+              const int4 pr = *reinterpret_cast<const int4*>(&sg.prow[st][ltid]);
               k = (int64_t)(((uint64_t)(uint32_t)pr.y << 32) | (uint32_t)pr.x);
               v = (int64_t)(((uint64_t)(uint32_t)pr.w << 32) | (uint32_t)pr.z);
             }
@@ -334,7 +375,7 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
             const unsigned landed =
               __reduce_and_sync(0xffffffffu, (uint32_t)((uint64_t)k ^ ((uint64_t)k >> 32) ^ (uint64_t)v ^
                                                         ((uint64_t)v >> 32)) | 1u);
-            if (lane == 0 && landed) mbar_arrive(&s.empty_probe[st]);
+            if (lane == 0 && landed) mbar_arrive(&sg.empty_probe[st]);
             q++;
 
             const uint32_t h    = slot_hash_i64(k);
@@ -370,21 +411,21 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
                   matched = true;
                   bpay    = brow[idx].pay;
                   if constexpr (marks_build(KIND)) {
-                    uint32_t* w      = &s.bmatch[bs][idx >> 5];
+                    uint32_t* w      = &sg.bmatch[idx >> 5];
                     const uint32_t b = 1u << (idx & 31);
                     if (!(*w & b)) atomicOr(w, b);
                   }
                 }
-                emit_outer_row<C>(s, d, cur, lane, found, k, bpay, k, v, kSideBuild | kSideProbe);
+                emit_outer_row<C>(sg, d, lane, found, k, bpay, k, v, kSideBuild | kSideProbe);
                 if (found) slot = (slot + 1) & (C::kSlots - 1);  // multimap: scan past the hit
               }
               // the anti join's rule: a row is unmatched when no job of its bucket matched it
-              const int64_t prow_at = r0 + tid;
+              const int64_t prow_at = r0 + ltid;
               uint32_t* word        = d.probe_bits + (prow_at >> 5);
               const uint32_t bit    = 1u << (prow_at & 31);
               if (multi && matched && !last) atomicOr(word, bit);
               const bool lone = valid && !matched && last && (!multi || !(__ldcg(word) & bit));
-              emit_outer_row<C>(s, d, cur, lane, lone, 0, 0, k, v, kSideProbe);
+              emit_outer_row<C>(sg, d, lane, lone, 0, 0, k, v, kSideProbe);
               continue;
             }
             if constexpr (KIND == kSemi || KIND == kAnti) {
@@ -401,7 +442,7 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
                   slot = (slot + 1) & (C::kSlots - 1);
                 }
               }
-              const int64_t prow_at = r0 + tid;  // position of this row in the prepared probe side
+              const int64_t prow_at = r0 + ltid;  // position of this row in the prepared probe side
               uint32_t* word        = d.probe_bits + (prow_at >> 5);
               const uint32_t bit    = 1u << (prow_at & 31);
               bool emit;
@@ -417,24 +458,24 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
                 const int leader = __ffs(m) - 1;
                 int obase        = 0;
                 if (lane == leader) {
-                  obase = atomicAdd(&s.scnt[cur], __popc(m));
-                  if (obase >= C::kOutRows) atomicSub(&s.scnt[cur], __popc(m));
+                  obase = atomicAdd(&sg.scnt, __popc(m));
+                  if (obase >= C::kOutRows) atomicSub(&sg.scnt, __popc(m));
                 }
                 obase            = __shfl_sync(0xffffffffu, obase, leader);
                 const int pos    = obase + __popc(m & lanemask_lt());
                 const bool spill = emit && pos >= C::kOutRows;
                 if (emit && !spill) {
-                  s.sout[cur][0][pos] = k;
-                  s.sout[cur][1][pos] = v;
+                  sg.sout[0][pos] = k;
+                  sg.sout[1][pos] = v;
                 }
                 const unsigned ms = __ballot_sync(0xffffffffu, spill);
                 if (ms) {
                   const int sl = __ffs(ms) - 1;
-                  unsigned long long g = 0;
-                  if (lane == sl) g = atomicAdd(d.out_count, (unsigned long long)__popc(ms));
-                  g = __shfl_sync(0xffffffffu, g, sl);
+                  unsigned long long gc = 0;
+                  if (lane == sl) gc = atomicAdd(d.out_count, (unsigned long long)__popc(ms));
+                  gc = __shfl_sync(0xffffffffu, gc, sl);
                   if (spill) {
-                    const int64_t gi = (int64_t)g + __popc(ms & lanemask_lt());
+                    const int64_t gi = (int64_t)gc + __popc(ms & lanemask_lt());
                     if (gi < d.out_capacity) {
                       d.out[0][gi] = k;
                       d.out[1][gi] = v;
@@ -470,30 +511,30 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
               const int leader = __ffs(m) - 1;
               int obase        = 0;
               if (lane == leader) {
-                obase = atomicAdd(&s.scnt[cur], __popc(m));
+                obase = atomicAdd(&sg.scnt, __popc(m));
                 // a full tile stays "full": spilled matches are counted by the global counter below, so
                 // pull the tile counter back and keep it from ever wrapping (hot keys: > 2^31 matches)
-                if (obase >= C::kOutRows) atomicSub(&s.scnt[cur], __popc(m));
+                if (obase >= C::kOutRows) atomicSub(&sg.scnt, __popc(m));
               }
               obase         = __shfl_sync(0xffffffffu, obase, leader);
               const int pos = obase + __popc(m & lanemask_lt());
               const bool spill = found && pos >= C::kOutRows;
               if (found && !spill) {
-                s.sout[cur][0][pos] = k;
-                s.sout[cur][1][pos] = brow[idx].pay;
-                s.sout[cur][2][pos] = k;
-                s.sout[cur][3][pos] = v;
+                sg.sout[0][pos] = k;
+                sg.sout[1][pos] = brow[idx].pay;
+                sg.sout[2][pos] = k;
+                sg.sout[3][pos] = v;
               }
               // tile full (high selectivity / duplicates): the warp reserves its own run of
               // the output with one atomicAdd and stores it directly
               const unsigned ms = __ballot_sync(0xffffffffu, spill);
               if (ms) {
                 const int sl = __ffs(ms) - 1;
-                unsigned long long g = 0;
-                if (lane == sl) g = atomicAdd(d.out_count, (unsigned long long)__popc(ms));
-                g = __shfl_sync(0xffffffffu, g, sl);
+                unsigned long long gc = 0;
+                if (lane == sl) gc = atomicAdd(d.out_count, (unsigned long long)__popc(ms));
+                gc = __shfl_sync(0xffffffffu, gc, sl);
                 if (spill) {
-                  const int64_t gi = (int64_t)g + __popc(ms & lanemask_lt());
+                  const int64_t gi = (int64_t)gc + __popc(ms & lanemask_lt());
                   if (gi < d.out_capacity) {
                     d.out[0][gi] = k;
                     d.out[1][gi] = brow[idx].pay;
@@ -506,89 +547,69 @@ __global__ void __launch_bounds__(C::kThreads, 1) bucket_join_kernel(JoinDev d)
             }
           }
 
-          // ---- end of build job: table and row store are released, output tiles rotate
-          if (tid == 0 && pend_n) s.sbase[pend_tile] = pend_base_reg;
-          consumer_sync<kConsumers>();
+          // ---- end of build job: table, row store and output tile are released
+          group_sync<kConsumers>(g);
           if constexpr (KIND == kFullOuter) {
             // every probe row of the bucket has passed this job: its build rows with a clear bit match
-            // no left row.  They are read from the row store and appended to tile `cur`, so the store
-            // is released and the tile handed over only after a second barrier.
-            for (int r0 = tid - lane; r0 < nb; r0 += kConsumers) {
+            // no left row.  They are read from the row store and appended to the tile, so the store
+            // is released, the bits cleared and the tile handed over only after a second barrier.
+            for (int r0 = ltid - lane; r0 < nb; r0 += kConsumers) {
               const int r     = r0 + lane;
-              const bool lone = r < nb && !((s.bmatch[bs][r >> 5] >> (r & 31)) & 1u);
+              const bool lone = r < nb && !((sg.bmatch[r >> 5] >> (r & 31)) & 1u);
               int64_t bk = 0, bp = 0;
               if (lone) {
                 bk = brow[r].key;
                 bp = brow[r].pay;
               }
-              emit_outer_row<C>(s, d, cur, lane, lone, bk, bp, 0, 0, kSideBuild);
+              emit_outer_row<C>(sg, d, lane, lone, bk, bp, 0, 0, kSideBuild);
             }
-            consumer_sync<kConsumers>();
+            group_sync<kConsumers>(g);
+            for (int i = ltid; i < C::kBuildChunk / 32; i += kConsumers) sg.bmatch[i] = 0;
           }
           if constexpr (KIND == kMark) {
             // This job's matched bits move to the global array at the job's row position c0.  Thread i
-            // owns word i of bmatch[bs] from this barrier on: the job's atomicOrs all precede the
-            // barrier above, nothing sets a bit of bmatch[bs] again before the probe phase of job
-            // u + 2, and every thread reaches that phase only through job u + 1's two barriers, which
-            // this thread passes after the flush.  So a plain read and a plain store of 0 are
-            // ordered, no second barrier is needed, and the build phase does not clear bmatch for
-            // this kind.  Buckets start at any row, so a word straddles two global words, which
-            // neighbouring jobs (of this or another CTA) may share: atomicOr.
-            if (tid < C::kBuildChunk / 32) {
-              const uint32_t w = s.bmatch[bs][tid];
+            // owns word i of bmatch from the barrier above on: the job's atomicOrs all precede it, and
+            // the group sets a bit again only in the probe phase of its next job, which every thread
+            // reaches only through that job's two barriers before the probe, which this thread passes
+            // after the flush.  So a plain read and a plain store of 0 are ordered, and no other
+            // barrier is needed.  Buckets start at any row, so a word straddles two global words,
+            // which neighbouring jobs (of this or another group or CTA) may share: atomicOr.
+            if (ltid < C::kBuildChunk / 32) {
+              const uint32_t w = sg.bmatch[ltid];
               if (w) {
-                s.bmatch[bs][tid] = 0;
-                const int64_t at  = c0 + 32 * tid;
-                uint32_t* g       = d.build_bits + (at >> 5);
-                const int sh      = (int)(at & 31);
-                atomicOr(g, w << sh);
-                if (sh && (w >> (32 - sh))) atomicOr(g + 1, w >> (32 - sh));
+                sg.bmatch[ltid]  = 0;
+                const int64_t at = c0 + 32 * ltid;
+                uint32_t* gw     = d.build_bits + (at >> 5);
+                const int sh     = (int)(at & 31);
+                atomicOr(gw, w << sh);
+                if (sh && (w >> (32 - sh))) atomicOr(gw + 1, w >> (32 - sh));
               }
             }
           }
-          if (lane == 0) mbar_arrive(&s.empty_build[bs]);
-          if (pend_n) {
-            // copy out the tile whose atomicAdd was issued one build job ago (latency hidden);
-            // it stays untouched until the job after next, when every thread is past here
-            const int64_t gb = (int64_t)s.sbase[pend_tile];
-#pragma unroll
-            for (int c = 0; c < kCols; c++)
-              for (int i = tid; i < pend_n; i += kConsumers)
-                if (gb + i < d.out_capacity) d.out[c][gb + i] = s.sout[pend_tile][c][i];
-            if constexpr (kOuter)
-              for (int i = tid; i < pend_n; i += kConsumers)
-                if (gb + i < d.out_capacity) d.out_sides[gb + i] = s.ssides[pend_tile][i];
-            if (tid == 0) s.scnt[pend_tile] = 0;
-            pend_n = 0;
+          if (lane == 0) mbar_arrive(&sg.empty_build);
+          int n_out = sg.scnt;
+          if (n_out > C::kOutRows) n_out = C::kOutRows;
+          unsigned long long tile_base = 0;
+          if (ltid == 0 && n_out > 0) tile_base = atomicAdd(d.out_count, (unsigned long long)n_out);
+          // Clear the table for the group's next job.  Every probe of this job is past the barrier
+          // above, and the next job inserts only after its first barrier, which every thread reaches
+          // after its share of the clear.
+          {
+            uint4* t = reinterpret_cast<uint4*>(slots);
+            for (int i = ltid; i < C::kSlots / 4; i += kConsumers) t[i] = make_uint4(0, 0, 0, 0);
           }
-          int n_out = s.scnt[cur];
-          if (n_out > 0) {
-            if (n_out > C::kOutRows) n_out = C::kOutRows;
-            if (tid == 0) pend_base_reg = atomicAdd(d.out_count, (unsigned long long)n_out);
-            pend_n    = n_out;
-            pend_tile = cur;
-            cur       = cur + 1 == kOutTiles ? 0 : cur + 1;
-          }
+          if (ltid == 0 && n_out > 0) sg.sbase = tile_base;
+          pend_n = n_out;
           u++;
         }
       }
     }
   }
 
-  // ---- drain the pending tile (the current one is empty: every job hands its tile over)
+  // ---- copy out the last job's tile
   if (!is_producer) {
-    if (tid == 0 && pend_n) s.sbase[pend_tile] = pend_base_reg;
-    consumer_sync<kConsumers>();
-    if (pend_n) {
-      const int64_t gb = (int64_t)s.sbase[pend_tile];
-#pragma unroll
-      for (int c = 0; c < kCols; c++)
-        for (int i = tid; i < pend_n; i += kConsumers)
-          if (gb + i < d.out_capacity) d.out[c][gb + i] = s.sout[pend_tile][c][i];
-      if constexpr (kOuter)
-        for (int i = tid; i < pend_n; i += kConsumers)
-          if (gb + i < d.out_capacity) d.out_sides[gb + i] = s.ssides[pend_tile][i];
-    }
+    group_sync<kConsumers>(g);
+    if (pend_n) copy_out_tile<C, KIND>(sg, d, pend_n, ltid);
   }
 }
 
@@ -605,7 +626,8 @@ int join_shape()
 template <class C, int KIND>
 int launch_join(const JoinDev& d, int ctas_per_sm, cudaStream_t stream)
 {
-  const size_t smem = sizeof(JoinSmemOf<C, KIND>);
+  const size_t smem = sizeof(JoinSmem<C, KIND>);
+  static_assert(sizeof(JoinSmem<C, KIND>) <= 227 * 1024, "more shared memory than a block may use");
   auto kern         = bucket_join_kernel<C, KIND>;
   DJ_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = sm_count() * ctas_per_sm;
