@@ -280,7 +280,7 @@ static int load_all_kernels()
     return DJ_ERR_CUDA;
   }
   const void* anchors[] = {(const void*)verdict_kernel, dj::partition_module_kernel(), dj::join_module_kernel(),
-                           dj::generate_module_kernel()};
+                           dj::generate_module_kernel(), dj::broadcast_module_kernel()};
   for (const void* a : anchors) {
     cudaFunction_t f = nullptr;
     DJ_CUDA_TRY(cudaGetFuncBySymbol(&f, a));
@@ -829,6 +829,92 @@ static double ms_since(std::chrono::high_resolution_clock::time_point t0)
   return std::chrono::duration<double, std::milli>(std::chrono::high_resolution_clock::now() - t0).count();
 }
 
+// Words 3..12 of a join's hello: whether peers can map this rank's workspace (3), its offset inside its
+// allocation (4) and the allocation's CUDA IPC handle (5..12).
+static void workspace_identity(dj_comm* comm, void* d_workspace, int64_t* hello)
+{
+  if (comm->peer_ok && comm->group) {
+    // one address space: the raw workspace pointer stands in for the IPC handle (offset 0)
+    hello[3] = 1;
+    memcpy(&hello[5], &d_workspace, sizeof(d_workspace));
+  } else if (comm->peer_ok) {
+    CUdeviceptr base = 0;
+    size_t alloc_sz  = 0;
+    cudaIpcMemHandle_t wh;
+    memset(&wh, 0, sizeof(wh));
+    const bool ok = comm->fn_addr_range(&base, &alloc_sz, (CUdeviceptr)d_workspace) == CUDA_SUCCESS &&
+                    cudaIpcGetMemHandle(&wh, (void*)base) == cudaSuccess;
+    cudaGetLastError();
+    hello[3] = ok ? 1 : 0;
+    hello[4] = ok ? (int64_t)((CUdeviceptr)d_workspace - base) : 0;
+    memcpy(&hello[5], &wh, 64);
+  }
+}
+
+// Maps every peer's join workspace, described by the call's hello (ipc ok at word 3, offset in the
+// allocation at word 4, handle at words 5..12 of every rank's `hello_words`).  Mappings are cached per
+// allocation; a peer whose allocation changed since the last call has its old mapping closed first,
+// and then every rank agrees that the new mappings worked before anybody pushes.  *use_peer comes in as
+// this call's wish for the copy-engine exchange and goes out as the collective decision; peer_ws[r] is
+// rank r's workspace as seen from here (nullptr for this rank, or without the peer exchange).
+static int map_peer_workspaces(dj_comm* comm, const std::vector<int64_t>& hello, int hello_words, bool* use_peer,
+                               std::vector<char*>* peer_ws)
+{
+  const int world = comm->size, rank = comm->rank;
+  auto H = [&](int r, int f) -> int64_t { return hello[(size_t)r * hello_words + f]; };
+  for (int r = 0; r < world; r++) *use_peer = *use_peer && H(r, 3) == 1;
+  peer_ws->assign(world, nullptr);
+  if (!*use_peer) return DJ_OK;
+  bool any_new = false;  // identical on every rank: everybody sees the same handles
+  if (comm->last_handle.size() != (size_t)world * 8) {
+    comm->last_handle.assign((size_t)world * 8, 0);
+    any_new = true;
+  }
+  for (int r = 0; r < world; r++)
+    if (memcmp(&comm->last_handle[(size_t)r * 8], &hello[(size_t)r * hello_words + 5], 64) != 0) any_new = true;
+  int64_t mapped = 1;
+  for (int r = 0; r < world && mapped; r++) {
+    if (r == rank) continue;
+    cudaIpcMemHandle_t h;
+    memcpy(&h, &hello[(size_t)r * hello_words + 5], 64);
+    (*peer_ws)[r] = map_peer_workspace(comm, r, h, H(r, 4));
+    if (!(*peer_ws)[r]) mapped = 0;
+  }
+  if (any_new) {
+    // a mapping was (re)opened somewhere: agree that it worked before anybody pushes
+    std::vector<int64_t> oks(world);
+    int rc = ctrl_gather_host(comm, kBankAck, &mapped, 1, oks.data());
+    if (rc) return rc;
+    for (int r = 0; r < world; r++) *use_peer = *use_peer && oks[r] == 1;
+    for (int r = 0; r < world; r++)
+      memcpy(&comm->last_handle[(size_t)r * 8], &hello[(size_t)r * hello_words + 5], 64);
+  } else if (!mapped) {
+    set_error("join exchange: a cached peer mapping disappeared");
+    return DJ_ERR_CUDA;
+  }
+  return DJ_OK;
+}
+
+// The collective overflow verdict over peer memory: a one-thread kernel stores this rank's verdict into
+// every peer's flag block over NVLink, the stream waits for the peers' words, and their words are
+// copied to h_res[1..] (4 bytes per rank) behind the wait.  The caller's one synchronisation of `st`
+// then returns the count and every verdict.
+static int post_and_await_verdicts(dj_comm* comm, cudaStream_t st, const int64_t* d_count, int64_t out_capacity,
+                                   uint32_t seq, int64_t* h_res)
+{
+  verdict_kernel<<<1, 32, 0, st>>>((const unsigned long long*)d_count, (unsigned long long)out_capacity,
+                                   comm->d_peer_flags, comm->size, comm->rank, kFlagSlots, kFlagSlots - 1, seq);
+  DJ_LAUNCH_CHECK();
+  for (int src = 0; src < comm->size; src++) {
+    if (src == comm->rank) continue;
+    int rc = stream_wait_flag(comm, st, comm->d_flags + (size_t)src * kFlagSlots + (kFlagSlots - 1), seq << 1);
+    if (rc) return rc;
+  }
+  DJ_CUDA_TRY(cudaMemcpy2DAsync(h_res + 1, 4, comm->d_flags + (kFlagSlots - 1), (size_t)kFlagSlots * 4, 4, comm->size,
+                                cudaMemcpyDeviceToHost, st));
+  return DJ_OK;
+}
+
 // The distributed join of every kind.  kind 0: inner join, out = (left key, left payload, right key,
 // right payload).  DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI: the right table's key column is passed as its
 // payload too (d_right_payload == d_right_key), it is always the build side, and out[0..1] receive
@@ -952,22 +1038,7 @@ static int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key
   {
     int64_t mine[kHello] = {nleft, nright, (int64_t)workspace_bytes, 0, 0};
     mine[13]             = kind;
-    if (comm->peer_ok && comm->group) {
-      // one address space: the raw workspace pointer stands in for the IPC handle (offset 0)
-      mine[3] = 1;
-      memcpy(&mine[5], &d_workspace, sizeof(d_workspace));
-    } else if (comm->peer_ok) {
-      CUdeviceptr base = 0;
-      size_t alloc_sz  = 0;
-      cudaIpcMemHandle_t wh;
-      memset(&wh, 0, sizeof(wh));
-      const bool ok = comm->fn_addr_range(&base, &alloc_sz, (CUdeviceptr)d_workspace) == CUDA_SUCCESS &&
-                      cudaIpcGetMemHandle(&wh, (void*)base) == cudaSuccess;
-      cudaGetLastError();
-      mine[3] = ok ? 1 : 0;
-      mine[4] = ok ? (int64_t)((CUdeviceptr)d_workspace - base) : 0;
-      memcpy(&mine[5], &wh, 64);
-    }
+    workspace_identity(comm, d_workspace, mine);
     rc = ctrl_gather_host(comm, kBankHello, mine, kHello, hello.data());
     if (rc) return rc;
   }
@@ -1065,39 +1136,11 @@ static int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key
     }
   }
 
-  // ---- 0b. copy-engine exchange: map every peer's workspace (cached per allocation; a peer whose
-  //          allocation changed since the last call has its old mapping closed first)
+  // ---- 0b. copy-engine exchange: map every peer's workspace
   bool use_peer = comm->peer_ok && 2 * odf <= kDataSlots;
-  for (int r = 0; r < world; r++) use_peer = use_peer && H(r, 3) == 1;
-  std::vector<char*> peer_ws(world, nullptr);
-  if (use_peer) {
-    bool any_new = false;  // identical on every rank: everybody sees the same handles
-    if (comm->last_handle.size() != (size_t)world * 8) {
-      comm->last_handle.assign((size_t)world * 8, 0);
-      any_new = true;
-    }
-    for (int r = 0; r < world; r++)
-      if (memcmp(&comm->last_handle[(size_t)r * 8], &hello[(size_t)r * kHello + 5], 64) != 0) any_new = true;
-    int64_t mapped = 1;
-    for (int r = 0; r < world && mapped; r++) {
-      if (r == rank) continue;
-      cudaIpcMemHandle_t h;
-      memcpy(&h, &hello[(size_t)r * kHello + 5], 64);
-      peer_ws[r] = map_peer_workspace(comm, r, h, H(r, 4));
-      if (!peer_ws[r]) mapped = 0;
-    }
-    if (any_new) {
-      // a mapping was (re)opened somewhere: agree that it worked before anybody pushes
-      std::vector<int64_t> oks(world);
-      rc = ctrl_gather_host(comm, kBankAck, &mapped, 1, oks.data());
-      if (rc) return rc;
-      for (int r = 0; r < world; r++) use_peer = use_peer && oks[r] == 1;
-      for (int r = 0; r < world; r++) memcpy(&comm->last_handle[(size_t)r * 8], &hello[(size_t)r * kHello + 5], 64);
-    } else if (!mapped) {
-      set_error("distributed_inner_join: a cached peer mapping disappeared");
-      return DJ_ERR_CUDA;
-    }
-  }
+  std::vector<char*> peer_ws;
+  rc = map_peer_workspaces(comm, hello, kHello, &use_peer, &peer_ws);
+  if (rc) return rc;
   if (!use_peer && !comm->nccl) {  // identical on every rank: nothing has been queued but the count reset
     set_error("distributed_inner_join: this exchange (odf %d; peer memory carries at most %d) needs NCCL, which a "
               "local group does not have", odf, kDataSlots / 2);
@@ -1502,20 +1545,12 @@ static int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key
   int64_t* h_res = comm->h_pinned + (128 << 10);
   if (use_peer) {
     trace.mark("verdict begin", st);
-    verdict_kernel<<<1, 32, 0, st>>>((const unsigned long long*)d_count, (unsigned long long)out_capacity,
-                                     comm->d_peer_flags, world, rank, kFlagSlots, kFlagSlots - 1, seq);
-    DJ_LAUNCH_CHECK();
-    for (int src = 0; src < G; src++) {
-      if (src == rank) continue;
-      rc = stream_wait_flag(comm, st, comm->d_flags + (size_t)src * kFlagSlots + (kFlagSlots - 1), seq << 1);
-      if (rc) {
-        drain_exchange();
-        return rc;
-      }
+    rc = post_and_await_verdicts(comm, st, d_count, out_capacity, seq, h_res);
+    if (rc) {
+      drain_exchange();
+      return rc;
     }
     trace.mark("verdicts received", st);
-    DJ_CUDA_TRY(cudaMemcpy2DAsync(h_res + 1, 4, comm->d_flags + (kFlagSlots - 1), (size_t)kFlagSlots * 4, 4, world,
-                                  cudaMemcpyDeviceToHost, st));
   }
   DJ_CUDA_TRY(cudaMemcpyAsync(h_res, d_count, 8, cudaMemcpyDeviceToHost, st));
   DJ_CUDA_TRY(cudaStreamSynchronize(st));
@@ -2033,4 +2068,285 @@ extern "C" int dj_distributed_outer_join_i64_host(dj_comm_t* comm, int kind, con
   int64_t* h[4] = {h_out_lk, h_out_lp, h_out_rk, h_out_rp};
   return host_join(comm, kind, h_left_key, h_left_payload, nleft, h_right_key, h_right_payload, nright, h,
                    h_out_sides, out_capacity, h_out_count, opts, d_workspace, workspace_bytes, stream);
+}
+
+// ------------------------------------------------------------------------- broadcast join
+
+// Word 13 of a broadcast join's hello: the kind plus a tag no repartitioned join sends, so that a rank
+// inside dj_broadcast_join_i64 and a rank inside a repartitioned join both see a kind mismatch in the
+// one hello they both sent, and both return DJ_ERR_ARG.
+constexpr int64_t kBroadcastKindTag = 0x100;
+constexpr int kBroadcastFlagSlot    = 0;  // data flag: "my right slice has landed in your workspace"
+
+// Workspace of a broadcast join, a pure function of (nleft, R = gathered right rows): count[32] |
+// gathered right keys [R] | gathered right payloads [R] | local join scratch.  Every rank's gathered
+// columns sit at the same offsets, so every rank knows where its slice goes inside every peer (element
+// offset: the right rows of the ranks before it), and every rank can check every rank's fit.
+struct BroadcastLayout {
+  size_t count, grk, grp, scratch, need;
+};
+static BroadcastLayout broadcast_layout(int64_t nl, int64_t R)
+{
+  BroadcastLayout L{};
+  Arena va(reinterpret_cast<void*>(4096), ~(size_t)0 >> 1);  // offsets only
+  auto off  = [&](const void* p) { return (size_t)((const char*)p - va.base); };
+  L.count   = off(va.take<int64_t>(32));
+  L.grk     = off(va.take<int64_t>((size_t)R));
+  L.grp     = off(va.take<int64_t>((size_t)R));
+  L.scratch = align_up(va.used, 256);
+  const size_t join = R <= DJ_BROADCAST_TABLE_MAX_ROWS
+                        ? broadcast_table_bytes(R)
+                        : std::max(local_join_workspace(R, nl), local_filter_join_workspace(nl, R)) + 8192;
+  L.need = L.scratch + join;
+  return L;
+}
+
+extern "C" size_t dj_broadcast_join_workspace_bytes(int64_t nleft, int64_t nright_total)
+{
+  return broadcast_layout(std::max<int64_t>(nleft, 0), std::max<int64_t>(nright_total, 0)).need;
+}
+
+// The local join of a broadcast join, chosen from R alone so that every rank takes the same path: the
+// hash table while it is small enough to stay in L2, else the radix-partitioned join of that kind with
+// the gathered right table as the build side (out = left ++ right).
+static int broadcast_local_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* grk,
+                                const int64_t* grp, int64_t R, int64_t* const out[4], uint8_t* out_sides,
+                                int64_t out_capacity, int64_t* d_count, Arena& arena, cudaStream_t st)
+{
+  if (R <= DJ_BROADCAST_TABLE_MAX_ROWS)
+    return broadcast_hash_join(kind, lk, lp, nl, grk, grp, R, out, out_sides, out_capacity, d_count, arena, st);
+  if (nl == 0) return DJ_OK;
+  if (kind == DJ_JOIN_LEFT_OUTER)
+    return local_outer_join(kind, lk, lp, nl, grk, grp, R, out, out_sides, out_capacity, d_count, arena, st);
+  if (kind) return local_filter_join(kind, lk, lp, nl, grk, R, out[0], out[1], out_capacity, d_count, arena, st);
+  return local_join(grk, grp, R, lk, lp, nl, out, out_capacity, d_count, true, arena, st);
+}
+
+// Every rank all-gathers the right table into the same place of its workspace and joins its own left
+// rows against it.  Steps: one hello (sizes, workspace, kind), the fit verdict from the layout, the
+// peer mappings, the pushes of this rank's right slice into every peer (copy engines and a data flag,
+// or grouped NCCL), the local join once every slice has landed, and the overflow verdict.
+static int broadcast_join(dj_comm_t* comm, int kind, const int64_t* d_left_key, const int64_t* d_left_payload,
+                          int64_t nleft, const int64_t* d_right_key, const int64_t* d_right_payload, int64_t nright,
+                          int64_t* const out[4], uint8_t* d_out_sides, int64_t out_capacity, int64_t* h_out_count,
+                          dj_join_options* opts, void* d_workspace, size_t workspace_bytes, cudaStream_t st)
+{
+  const bool filter = kind_is_filter(kind);
+  const int world   = comm ? comm->size : 1;
+  const int rank    = comm ? comm->rank : 0;
+  const size_t row_bytes = filter ? 8 : 16;  // the key column, and the payload column unless semi / anti
+  if (opts) {
+    opts->t_partition_ms = opts->t_comm_ms = opts->t_join_ms = 0;
+    opts->bytes_sent = opts->workspace_needed = 0;
+    opts->t_exchange_ms[0] = opts->t_exchange_ms[1] = 0;
+    opts->t_exchange_total_ms = 0;
+  }
+  char* wsb = (char*)d_workspace;
+  auto count_result = [&](int64_t n) -> int {
+    *h_out_count = n;
+    if (n <= out_capacity) return DJ_OK;
+    set_error("join output needs %lld rows, capacity %lld", (long long)n, (long long)out_capacity);
+    return DJ_ERR_OVERFLOW;
+  };
+
+  if (world == 1) {
+    DJ_REQUIRE(nright < ((int64_t)1 << 31), "broadcast_join: the right table is limited to 2^31 rows");
+    const BroadcastLayout L = broadcast_layout(nleft, nright);
+    if (workspace_bytes < L.need) {
+      if (opts) opts->workspace_needed = (int64_t)L.need;
+      set_error("broadcast_join: workspace too small (%zu of %zu bytes)", workspace_bytes, L.need);
+      return DJ_ERR_WORKSPACE;
+    }
+    int64_t* d_count = (int64_t*)(wsb + L.count);
+    int64_t* grk     = (int64_t*)(wsb + L.grk);
+    int64_t* grp     = filter ? grk : (int64_t*)(wsb + L.grp);
+    DJ_CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), st));
+    if (nright > 0) {
+      DJ_CUDA_TRY(cudaMemcpyAsync(grk, d_right_key, (size_t)nright * 8, cudaMemcpyDeviceToDevice, st));
+      if (!filter)
+        DJ_CUDA_TRY(cudaMemcpyAsync(grp, d_right_payload, (size_t)nright * 8, cudaMemcpyDeviceToDevice, st));
+    }
+    Arena arena(wsb + L.scratch, workspace_bytes - L.scratch);
+    int rc = broadcast_local_join(kind, d_left_key, d_left_payload, nleft, grk, grp, nright, out, d_out_sides,
+                                  out_capacity, d_count, arena, st);
+    if (rc) return rc;
+    int64_t n = 0;
+    DJ_CUDA_TRY(cudaMemcpyAsync(&n, d_count, 8, cudaMemcpyDeviceToHost, st));
+    DJ_CUDA_TRY(cudaStreamSynchronize(st));
+    return count_result(n);
+  }
+
+  DJ_REQUIRE(((uintptr_t)d_workspace & 255) == 0, "broadcast_join: the workspace must be 256-byte aligned");
+  // ---- hello: every rank's table sizes, workspace size and identity, and kind
+  constexpr int kHello = 14;
+  std::vector<int64_t> hello((size_t)world * kHello);
+  {
+    int64_t mine[kHello] = {nleft, nright, (int64_t)workspace_bytes, 0, 0};
+    mine[13]             = kBroadcastKindTag + kind;
+    workspace_identity(comm, d_workspace, mine);
+    int rc = ctrl_gather_host(comm, kBankHello, mine, kHello, hello.data());
+    if (rc) return rc;
+  }
+  auto H = [&](int r, int f) -> int64_t { return hello[(size_t)r * kHello + f]; };
+  for (int r = 0; r < world; r++)
+    if (H(r, 13) != kBroadcastKindTag + kind) {  // identical verdict everywhere; nothing is queued
+      set_error("broadcast join: rank %d asked for %s join kind %lld, this rank for broadcast join kind %d", r,
+                H(r, 13) >= kBroadcastKindTag ? "broadcast" : "repartitioned",
+                (long long)(H(r, 13) >= kBroadcastKindTag ? H(r, 13) - kBroadcastKindTag : H(r, 13)), kind);
+      return DJ_ERR_ARG;
+    }
+  int64_t R = 0, before = 0;  // gathered right rows, and those of the ranks before this one
+  for (int r = 0; r < world; r++) {
+    if (r < rank) before += H(r, 1);
+    R += H(r, 1);
+  }
+  DJ_REQUIRE(R < ((int64_t)1 << 31), "broadcast_join: the gathered right table (%lld rows) is limited to 2^31 rows",
+             (long long)R);
+  const BroadcastLayout L = broadcast_layout(nleft, R);
+  for (int r = 0; r < world; r++) {
+    const size_t need = broadcast_layout(H(r, 0), R).need;
+    if (need > (size_t)H(r, 2)) {
+      if (opts) opts->workspace_needed = (int64_t)L.need;
+      set_error("broadcast_join: workspace too small on rank %d (%zu of %lld bytes; this rank needs %zu)", r, need,
+                (long long)H(r, 2), L.need);
+      return DJ_ERR_WORKSPACE;
+    }
+  }
+
+  // ---- peer mappings (copy-engine exchange) or NCCL
+  bool use_peer = comm->peer_ok;
+  std::vector<char*> peer_ws;
+  int rc = map_peer_workspaces(comm, hello, kHello, &use_peer, &peer_ws);
+  if (rc) return rc;
+  if (!use_peer && !comm->nccl) {  // identical on every rank: nothing has been queued
+    set_error("broadcast_join: the exchange needs peer memory or NCCL, and a local group has no NCCL");
+    return DJ_ERR_ARG;
+  }
+  const uint32_t seq = use_peer ? ++comm->seq : 0;
+  int64_t* d_count   = (int64_t*)(wsb + L.count);
+  int64_t* grk       = (int64_t*)(wsb + L.grk);
+  int64_t* grp       = filter ? grk : (int64_t*)(wsb + L.grp);
+  DJ_CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), st));
+
+  // ---- this rank's right slice into every rank's gathered columns, at element offset `before`
+  const int64_t* src_cols[2] = {d_right_key, d_right_payload};
+  const size_t dst_off[2]    = {L.grk, L.grp};
+  const int ncols            = filter ? 1 : 2;
+  for (int c = 0; c < ncols && nright > 0; c++)
+    DJ_CUDA_TRY(cudaMemcpyAsync(wsb + dst_off[c] + (size_t)before * 8, src_cols[c], (size_t)nright * 8,
+                                cudaMemcpyDeviceToDevice, st));
+  auto drain_pushes = [&]() {
+    if (use_peer)
+      for (int i = 0; i < world; i++)
+        if (i != rank) cudaStreamSynchronize(comm->peer_stream[i]);
+  };
+  if (use_peer) {
+    DJ_CUDA_TRY(cudaEventRecord(comm->ev_ready, st));  // the caller's right columns are ready
+    // destinations in rank+1, rank+2, ... order, as in the repartitioned exchange: no receiver sees
+    // every sender at once
+    for (int k = 1; k < world; k++) {
+      const int i     = (rank + k) % world;
+      cudaStream_t ps = comm->peer_stream[i];
+      DJ_CUDA_TRY(cudaStreamWaitEvent(ps, comm->ev_ready, 0));
+      for (int c = 0; c < ncols && nright > 0; c++)
+        DJ_CUDA_TRY(cudaMemcpyAsync(peer_ws[i] + dst_off[c] + (size_t)before * 8, src_cols[c], (size_t)nright * 8,
+                                    cudaMemcpyDefault, ps));
+      uint32_t* flag = comm->peer_flags[i] + (size_t)rank * kFlagSlots + kBroadcastFlagSlot;
+      if (!comm->flag_by_memcpy && comm->fn_write32((CUstream)ps, (CUdeviceptr)flag, seq, 0) != CUDA_SUCCESS)
+        comm->flag_by_memcpy = true;
+      if (comm->flag_by_memcpy) {
+        // 4-byte copy from a pinned word (ordered behind the data copies on the same stream)
+        uint32_t* w = reinterpret_cast<uint32_t*>(comm->h_pinned + (900 << 10)) + (seq % 4096);
+        *w          = seq;
+        DJ_CUDA_TRY(cudaMemcpyAsync(flag, w, 4, cudaMemcpyDefault, ps));
+      }
+    }
+    for (int src = 0; src < world; src++) {
+      if (src == rank) continue;
+      if ((rc = stream_wait_flag(comm, st, comm->d_flags + (size_t)src * kFlagSlots + kBroadcastFlagSlot, seq))) {
+        drain_pushes();
+        return rc;
+      }
+    }
+  } else {
+    DJ_NCCL_TRY(ncclGroupStart());
+    for (int c = 0; c < ncols; c++) {
+      int64_t at = 0;  // first gathered row of rank i
+      for (int i = 0; i < world; at += H(i, 1), i++) {
+        if (i == rank) continue;
+        if (nright > 0) DJ_NCCL_TRY(ncclSend(src_cols[c], (size_t)nright * 8, ncclInt8, i, comm->nccl, st));
+        if (H(i, 1) > 0)
+          DJ_NCCL_TRY(ncclRecv(wsb + dst_off[c] + (size_t)at * 8, (size_t)H(i, 1) * 8, ncclInt8, i, comm->nccl, st));
+      }
+    }
+    DJ_NCCL_TRY(ncclGroupEnd());
+  }
+  if (opts) opts->bytes_sent = (int64_t)(world - 1) * nright * (int64_t)row_bytes;
+
+  // ---- local join of this rank's left rows against the gathered right table
+  Arena arena(wsb + L.scratch, workspace_bytes - L.scratch);
+  rc = broadcast_local_join(kind, d_left_key, d_left_payload, nleft, grk, grp, R, out, d_out_sides, out_capacity,
+                            d_count, arena, st);
+  if (rc) {
+    drain_pushes();
+    return rc;
+  }
+
+  // ---- overflow verdict.  Besides agreeing on DJ_ERR_OVERFLOW, it keeps a fast rank from pushing the
+  //      NEXT call's right slice into a peer that is still probing this call's gathered columns: a
+  //      rank's verdict is posted behind its join on its stream, and no rank returns before it has
+  //      received every peer's verdict.
+  int64_t* h_res = comm->h_pinned + (128 << 10);
+  if (use_peer && (rc = post_and_await_verdicts(comm, st, d_count, out_capacity, seq, h_res))) {
+    drain_pushes();
+    return rc;
+  }
+  DJ_CUDA_TRY(cudaMemcpyAsync(h_res, d_count, 8, cudaMemcpyDeviceToHost, st));
+  DJ_CUDA_TRY(cudaStreamSynchronize(st));
+  drain_pushes();  // the caller may reuse its right columns once the call returns
+  const int64_t n = h_res[0];
+  int over_rank   = n > out_capacity ? rank : -1;
+  if (use_peer) {
+    const uint32_t* hv = reinterpret_cast<const uint32_t*>(h_res + 1);
+    for (int r = 0; r < world; r++)
+      if (r != rank && (hv[r] & 1u)) over_rank = r;
+  } else {
+    int64_t over = n > out_capacity ? 1 : 0;
+    std::vector<int64_t> overs(world);
+    if ((rc = ctrl_allgather(comm, &over, 1, overs.data()))) return rc;
+    for (int r = 0; r < world; r++)
+      if (overs[r]) over_rank = r;
+  }
+  *h_out_count = n;
+  if (over_rank >= 0) {
+    set_error("join output does not fit on rank %d (this rank: %lld rows, capacity %lld)", over_rank, (long long)n,
+              (long long)out_capacity);
+    return DJ_ERR_OVERFLOW;
+  }
+  return DJ_OK;
+}
+
+extern "C" int dj_broadcast_join_i64(dj_comm_t* comm, int kind, const int64_t* d_left_key,
+                                     const int64_t* d_left_payload, int64_t nleft, const int64_t* d_right_key,
+                                     const int64_t* d_right_payload, int64_t nright, int64_t* d_out_lk,
+                                     int64_t* d_out_lp, int64_t* d_out_rk, int64_t* d_out_rp, uint8_t* d_out_sides,
+                                     int64_t out_capacity, int64_t* h_out_count, dj_join_options* opts,
+                                     void* d_workspace, size_t workspace_bytes, void* stream)
+{
+  DJ_REQUIRE(kind != DJ_JOIN_FULL_OUTER, "broadcast_join: a full outer join has no broadcast plan (a right row is "
+             "unmatched only once every rank's matches are known)");
+  DJ_REQUIRE(kind == 0 || kind_is_filter(kind) || kind == DJ_JOIN_LEFT_OUTER, "broadcast_join: unknown join kind %d",
+             kind);
+  const bool filter = kind_is_filter(kind), outer = kind == DJ_JOIN_LEFT_OUTER;
+  DJ_REQUIRE(nleft >= 0 && nright >= 0 && out_capacity >= 0 && h_out_count && d_workspace,
+             "broadcast_join: bad argument");
+  DJ_REQUIRE((nleft == 0 || (d_left_key && d_left_payload)) &&
+               (nright == 0 || (d_right_key && (filter || d_right_payload))),
+             "broadcast_join: bad input columns");
+  DJ_REQUIRE(out_capacity == 0 || (d_out_lk && d_out_lp && (filter || (d_out_rk && d_out_rp && (!outer || d_out_sides)))),
+             "broadcast_join: bad output columns");
+  int64_t* const out[4] = {d_out_lk, d_out_lp, d_out_rk, d_out_rp};
+  return broadcast_join(comm, kind, d_left_key, d_left_payload, nleft, d_right_key, d_right_payload, nright, out,
+                        d_out_sides, out_capacity, h_out_count, opts, d_workspace, workspace_bytes,
+                        (cudaStream_t)stream);
 }

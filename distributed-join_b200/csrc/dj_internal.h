@@ -262,10 +262,21 @@ int local_outer_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl,
                      int64_t nr, int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
                      Arena& arena, cudaStream_t stream);
 
-// One kernel of each translation unit's module (partition.cu, join.cu, generate.cu): comm.cu
-// loads every function of these modules before ranks can wait on each other.
+// Broadcast join's local join (broadcast.cu): a hash table of the distinct keys of the right table
+// (rk, rp)[nr], nr <= DJ_BROADCAST_TABLE_MAX_ROWS, probed by the left columns (lk, lp)[nl] in place.
+// kind 0 / DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI / DJ_JOIN_LEFT_OUTER; out and out_sides as for the
+// repartitioned join of that kind (rp, out[2..3] and out_sides unused by semi / anti); appends at the
+// running *d_out_count.  Takes broadcast_table_bytes(nr) from `arena`.
+size_t broadcast_table_bytes(int64_t nr);
+int broadcast_hash_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* rk,
+                        const int64_t* rp, int64_t nr, int64_t* const out[4], uint8_t* out_sides,
+                        int64_t out_capacity, int64_t* d_out_count, Arena& arena, cudaStream_t stream);
+
+// One kernel of each translation unit's module (partition.cu, join.cu, generate.cu, broadcast.cu):
+// comm.cu loads every function of these modules before ranks can wait on each other.
 const void* partition_module_kernel();
 const void* join_module_kernel();
 const void* generate_module_kernel();
+const void* broadcast_module_kernel();
 
 }  // namespace dj

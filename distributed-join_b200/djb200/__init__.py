@@ -33,6 +33,7 @@ JOIN_LEFT_OUTER = 3
 JOIN_FULL_OUTER = 4
 SIDE_LEFT = 1  # bits of an outer join's `sides` column: which side of an output row is present
 SIDE_RIGHT = 2
+BROADCAST_TABLE_MAX_ROWS = 1 << 20  # dj_b200.h: gathered right rows up to which the broadcast join's hash table runs
 
 
 class DjError(RuntimeError):
@@ -84,6 +85,7 @@ ABI_SYMBOLS = [
     "dj_distributed_outer_join_workspace_bytes", "dj_distributed_outer_join_i64",
     "dj_distributed_left_filter_join_host_workspace_bytes", "dj_distributed_left_filter_join_i64_host",
     "dj_distributed_outer_join_host_workspace_bytes", "dj_distributed_outer_join_i64_host",
+    "dj_broadcast_join_workspace_bytes", "dj_broadcast_join_i64",
 ]
 
 _lib = None
@@ -149,6 +151,9 @@ def lib() -> C.CDLL:
         fn.argtypes = [i64, i64, i64, C.c_int, C.c_int]
     L.dj_distributed_left_filter_join_i64_host.argtypes = L.dj_distributed_left_filter_join_i64.argtypes
     L.dj_distributed_outer_join_i64_host.argtypes = L.dj_distributed_outer_join_i64.argtypes
+    L.dj_broadcast_join_workspace_bytes.restype = sz
+    L.dj_broadcast_join_workspace_bytes.argtypes = [i64, i64]
+    L.dj_broadcast_join_i64.argtypes = L.dj_distributed_outer_join_i64.argtypes
     L.dj_comm_create_local_group.argtypes = [C.c_int, C.POINTER(vp)]
     L.dj_testing_radix_repairs.argtypes = [C.POINTER(i64)]
     _lib = L
@@ -504,6 +509,39 @@ def distributed_full_outer_join(comm, lk, lp, rk, rp, odf=1, capacity=None, ws=N
     """SQL FULL OUTER JOIN: the left outer join plus every right row without a match once: see
     distributed_outer_join."""
     return distributed_outer_join(comm, JOIN_FULL_OUTER, lk, lp, rk, rp, odf, capacity, ws, outs)
+
+
+def distributed_broadcast_join(comm, kind, lk, lp, rk, rp=None, capacity=None, ws=None, outs=None):
+    """Broadcast join through dj_broadcast_join_i64: every rank all-gathers the right table and joins its
+    OWN left rows (lk, lp), which never move, against the union of every rank's right rows.  kind 0
+    (inner), JOIN_LEFT_SEMI / JOIN_LEFT_ANTI (rp may be None) or JOIN_LEFT_OUTER.  Returns a JoinResult
+    with 4 columns (inner), 2 (semi / anti: the kept left rows) or 5 (left outer: the sides column too),
+    trimmed.  The workspace is sized from the gathered right rows; `outs`: caller-owned columns for the
+    first attempt.  Both retry loops are collective, as for the repartitioned joins."""
+    filter_ = kind in (JOIN_LEFT_SEMI, JOIN_LEFT_ANTI)
+    lk, lp, rk = map(_i64dev, (lk, lp, rk))
+    if rp is not None:
+        rp = _i64dev(rp)
+    nl, nr = lk.numel(), rk.numel()
+    world = comm.size if comm else 1
+    if capacity is None:
+        capacity = max(nl, 1)
+    ncols = 2 if filter_ else 5 if kind == JOIN_LEFT_OUTER else 4
+
+    def call(outs, capacity, ws):
+        cnt = C.c_int64(0)
+        opts = JoinOptions(1, 0)
+        o = [_ptr(c) for c in outs] + [None] * (5 - len(outs))
+        rc = lib().dj_broadcast_join_i64(comm.handle if comm else None, kind, _ptr(lk), _ptr(lp), nl, _ptr(rk),
+                                         _ptr(rp), nr, *o, capacity, C.byref(cnt), C.byref(opts), _ptr(ws),
+                                         ws.numel(), _stream())
+        return rc, cnt.value, opts
+
+    ws_bytes = None
+    if ws is None:
+        total_right = sum(comm.allgather_i64([nr])) if world > 1 else nr
+        ws_bytes = lib().dj_broadcast_join_workspace_bytes(nl, total_right)
+    return _collective_join(comm, call, ncols, capacity, ws, ws_bytes, outs, lk.device)
 
 
 def _host_join(comm, name, call, ws, ws_bytes):

@@ -336,6 +336,52 @@ int dj_distributed_outer_join_i64_host(dj_comm_t* comm, int kind,
                                        void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * dj_broadcast_join_i64 -- broadcast join of a large left table with a small right table (a fact table
+ * against a dimension table, or an IN (subquery) filter against a short key list).  Instead of
+ * hash-partitioning both tables over the ranks, every rank all-gathers the right table over NVLink and
+ * joins ITS OWN left rows, as passed, against the union of every rank's right rows: left rows never
+ * move and are never radix-partitioned.
+ *   - kind 0: inner join; outputs (left key, left payload, right key, right payload), duplicate keys
+ *     give all pairs.
+ *   - DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI: outputs d_out_lk, d_out_lp only, each left row at most
+ *     once; d_right_payload, d_out_rk, d_out_rp and d_out_sides may be NULL.
+ *   - DJ_JOIN_LEFT_OUTER: the four columns plus d_out_sides, as dj_distributed_outer_join_i64 writes
+ *     them (3 for a pair, 1 with zeroed right columns for a left row without a match).
+ *   - DJ_JOIN_FULL_OUTER and any other kind: DJ_ERR_ARG on every rank before anything is exchanged
+ *     (a right row is unmatched only once every rank's match bits are known).
+ * Placement: rank r returns the join of its own left rows with the gathered right table, in
+ * unspecified row order; the union over the ranks is the global join.  This differs from the
+ * repartitioned joins, which place rows by murmur3 owner.  comm NULL or size 1: a local join of the
+ * same kind.  A right table empty on every rank gives nothing for inner and semi joins and every left
+ * row for anti (and, with sides 1, left outer) joins; a rank with no left rows returns 0 rows but
+ * still takes part in the exchange and the verdict.
+ * Collective behaviour is that of the repartitioned joins: every rank must pass the same kind
+ * (otherwise every rank returns DJ_ERR_ARG, also when a peer is inside a repartitioned join at the
+ * same time); a workspace short on any rank gives DJ_ERR_WORKSPACE on every rank with
+ * opts->workspace_needed set to this rank's need; an output that overflows on any rank gives
+ * DJ_ERR_OVERFLOW on every rank with an exact *h_out_count, and nothing is written past out_capacity.
+ * opts->over_decom_factor is ignored; opts->bytes_sent is (size - 1) * nright * (8 for semi / anti,
+ * 16 otherwise).  The gathered right table holds at most 2^31 rows (DJ_ERR_ARG beyond).
+ * Local join: while the gathered right table has at most DJ_BROADCAST_TABLE_MAX_ROWS rows, one hash
+ * table of its distinct keys is built and the left columns are streamed through it once; beyond, the
+ * radix-partitioned local join of the same kind runs on (left, gathered right).  Every rank picks the
+ * same path.  The workspace query depends on nleft and the gathered row count only (any kind).
+ */
+/* Gathered right rows up to which the hash-table path runs.  Set by the L2 budget: at 2^20 rows the table
+ * is 40 MB of the H100's 50 MB L2 (2^21 would be 80 MB).  The crossover with the radix path lies above it:
+ * 400M left rows at N = 1 on an H100 80GB HBM3 (700 W), the hash table took 21.6 / 7.7 / 25.4 ms for
+ * inner / semi / left outer at 2^20 right rows against the radix path's 29.1 / 27.7 / 40.8 ms
+ * (DESIGN.md §5e). */
+enum { DJ_BROADCAST_TABLE_MAX_ROWS = 1 << 20 };
+size_t dj_broadcast_join_workspace_bytes(int64_t nleft, int64_t nright_total);
+int dj_broadcast_join_i64(dj_comm_t* comm, int kind,
+                          const int64_t* d_left_key, const int64_t* d_left_payload, int64_t nleft,
+                          const int64_t* d_right_key, const int64_t* d_right_payload, int64_t nright,
+                          int64_t* d_out_lk, int64_t* d_out_lp, int64_t* d_out_rk, int64_t* d_out_rp,
+                          uint8_t* d_out_sides, int64_t out_capacity, int64_t* h_out_count,
+                          dj_join_options* opts, void* d_workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Testing: an in-process rank group.  Creates `size` communicators (ranks 0..size-1) on the
  * current device in one process; comms[r] is meant to be driven by its own host thread.  The
  * multi-rank join runs unchanged from its first control message to its overflow verdict; only
