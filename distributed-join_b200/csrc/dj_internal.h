@@ -202,13 +202,13 @@ struct PreparedSide {
   const int64_t* d_end;
   int64_t cap_rows;  // length of the `rows` array (bucket gaps included)
 };
-RadixPlan plan_for(int64_t nbuild, bool any_segmented);
-size_t side_ws_bytes(int64_t span_rows, const RadixPlan& plan, int nseg);
-// Semi / anti / outer joins: the plan for `nright` build rows with at least kFilterMinBits bits, so that the
-// probe side is spread over every SM however small the right table is; and the bytes of the
-// probe-row bit array for a probe side spanning `span_rows` rows.
+// The radix plan of a local join of `kind` with `nbuild` build rows.  Semi / anti / outer joins get
+// at least kFilterMinBits bits, so that the probe side is spread over every SM however small the
+// right table is.
 constexpr int kFilterMinBits = 10;
-RadixPlan filter_plan(int64_t nright);
+RadixPlan join_plan(int kind, int64_t nbuild);
+size_t side_ws_bytes(int64_t span_rows, const RadixPlan& plan, int nseg);
+// bytes of the probe-row bit array of a semi / anti / outer join for a probe side spanning `span_rows` rows
 size_t filter_bits_bytes(int64_t span_rows, const RadixPlan& plan);
 
 // Simple bump allocator over a caller-provided device workspace.
@@ -231,36 +231,49 @@ struct Arena {
 
 int prepare_side(const TableInput& in, const RadixPlan& plan, PreparedSide* out, Arena& arena,
                  cudaStream_t stream);
-int join_prepared(const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
-                  int64_t* const out[4], int64_t out_capacity, int64_t* d_out_count, bool swap,
-                  cudaStream_t stream, int kind = 0, uint32_t* d_probe_bits = nullptr,
-                  uint8_t* out_sides = nullptr, uint32_t* d_build_bits = nullptr);
-// Semi / anti join of the probe side's rows against the build side's keys: zeroes the probe-row
-// bit array (taken from `arena`) and runs the join kernel of that kind; out = (key, payload).
-int filter_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
-                         int64_t* out_key, int64_t* out_pay, int64_t out_capacity, int64_t* d_out_count,
-                         Arena& arena, cudaStream_t stream);
-// Left / full outer join of the probe (left) side against the build (right) side: zeroes the
-// probe-row bit array (taken from `arena`) and runs the join kernel of that kind.  out = (left key,
-// left payload, right key, right payload), out_sides = DJ_SIDE_* bits of every row.  kind
-// kJoinFullOuterMark also takes d_build_bits, (build.cap_rows + 31) / 32 words zeroed once by the caller.
-int outer_join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
-                        int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
-                        Arena& arena, cudaStream_t stream, uint32_t* d_build_bits = nullptr);
-int local_join(const int64_t* bk, const int64_t* bp, int64_t nb, const int64_t* pk,
-               const int64_t* pp, int64_t np, int64_t* const out[4], int64_t out_capacity,
-               int64_t* d_out_count, bool swap, Arena& arena, cudaStream_t stream);
-size_t local_join_workspace(int64_t nb, int64_t np);
-// Single-GPU semi / anti join of (lk, lp)[nl] against the keys rk[nr]; both sides non-empty.
-int local_filter_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* rk, int64_t nr,
-                      int64_t* out_key, int64_t* out_pay, int64_t out_capacity, int64_t* d_out_count, Arena& arena,
-                      cudaStream_t stream);
-size_t local_filter_join_workspace(int64_t nl, int64_t nr);
-// Single-GPU left / full outer join of (lk, lp)[nl] with (rk, rp)[nr]; both sides non-empty.  Its
-// workspace is local_filter_join_workspace(nl, nr): the same plan, sides and probe-row bits.
-int local_outer_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* rk, const int64_t* rp,
-                     int64_t nr, int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
-                     Arena& arena, cudaStream_t stream);
+// The join kernel of `kind` over two prepared sides; appends at the running *d_out_count.  out is
+// (left key, left payload, right key, right payload); semi / anti joins write only out[0..1].  Every
+// kind but the inner join builds on the right table; the inner join does when `swap` is set.  Kinds
+// other than the inner join take their probe-row bit array from `arena` and zero it; outer joins
+// write every row's DJ_SIDE_* bits to out_sides, and kJoinFullOuterMark also takes d_build_bits,
+// (build.cap_rows + 31) / 32 words zeroed once by the caller.
+int join_prepared(int kind, const PreparedSide& build, const PreparedSide& probe, const RadixPlan& plan,
+                  int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count, bool swap,
+                  Arena& arena, cudaStream_t stream, uint32_t* d_build_bits = nullptr);
+// Single-GPU join of `kind` of (lk, lp)[nl] with (rk, rp)[nr], both non-empty; semi / anti joins pass
+// the right key column as rp.  The inner join builds on the right table when `build_right` is set,
+// every other kind always does.  Its workspace is local_join_workspace(kind, nbuild, nprobe).
+int local_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* rk, const int64_t* rp,
+               int64_t nr, int64_t* const out[4], uint8_t* out_sides, int64_t out_capacity, int64_t* d_out_count,
+               bool build_right, Arena& arena, cudaStream_t stream);
+size_t local_join_workspace(int kind, int64_t nbuild, int64_t nprobe);
+
+// Which side the hash tables of an inner join are built on.  The caller's LEFT table is the build side
+// (the reference's drivers pass the unique-key build table as `left`, benchmark/distributed_join.cu:266-283)
+// unless the right table is clearly smaller: received slices of equal-sized tables differ by a few rows
+// per rank, and letting that noise pick the side made some ranks build on the duplicate-laden probe
+// table (measured at N=2: 11.2 ms instead of 7.9 ms for the same join).
+inline bool build_on_right(int64_t nleft, int64_t nright) { return nright + nright / 8 < nleft; }
+
+// The ABI's join kinds: 0 (inner), DJ_JOIN_LEFT_SEMI / ANTI (two output columns, the right table is a
+// key column) and DJ_JOIN_LEFT_OUTER / FULL_OUTER (four columns and the sides bytes).
+inline bool kind_is_filter(int kind) { return kind == DJ_JOIN_LEFT_SEMI || kind == DJ_JOIN_LEFT_ANTI; }
+inline bool kind_is_outer(int kind) { return kind == DJ_JOIN_LEFT_OUTER || kind == DJ_JOIN_FULL_OUTER; }
+inline int kind_out_cols(int kind) { return kind_is_filter(kind) ? 2 : 4; }
+
+// The distributed join of every kind (comm.cu).  kind 0: out = (left key, left payload, right key,
+// right payload).  Semi / anti: d_right_payload == d_right_key, out[0..1] receive the kept left rows.
+// Outer: out as for the inner join, d_out_sides receives every row's DJ_SIDE_* bits.
+int distributed_join(dj_comm_t* comm, int kind, const int64_t* d_left_key, const int64_t* d_left_payload,
+                     int64_t nleft, const int64_t* d_right_key, const int64_t* d_right_payload, int64_t nright,
+                     int64_t* d_out_lk, int64_t* d_out_lp, int64_t* d_out_rk, int64_t* d_out_rp, uint8_t* d_out_sides,
+                     int64_t out_capacity, int64_t* h_out_count, dj_join_options* opts, void* d_workspace,
+                     size_t workspace_bytes, void* stream);
+// Zeroes every output field of a join's options (nullptr: none).
+void reset_opts(dj_join_options* opts);
+// A single-rank join's result of n rows: *h_out_count = n, DJ_ERR_OVERFLOW (with the error set) if it
+// exceeds out_capacity.
+int single_rank_result(int64_t n, int64_t out_capacity, int64_t* h_out_count);
 
 // Broadcast join's local join (broadcast.cu): a hash table of the distinct keys of the right table
 // (rk, rp)[nr], nr <= DJ_BROADCAST_TABLE_MAX_ROWS, probed by the left columns (lk, lp)[nl] in place.
