@@ -1743,15 +1743,26 @@ extern "C" int dj_distributed_outer_join_i64(dj_comm_t* comm, int kind, const in
 // ------------------------------------------------------------------------- broadcast join
 
 constexpr int kBroadcastFlagSlot = 0;  // data flag: "my right slice has landed in your workspace"
+constexpr int kBroadcastBitsFlagSlot = 1;  // full outer: "my match bits for your slice have landed"
+
+// Words of a full outer join's match bits that cover the gathered rows [before, before + n): the words
+// [before >> 5, (before + n + 31) >> 5), none for an empty slice.  At most (n + 31) / 32 + 1 words,
+// because a slice generally starts inside a word.
+static int64_t slice_bit_words(int64_t before, int64_t n) { return n ? ((before + n + 31) >> 5) - (before >> 5) : 0; }
 
 // Workspace of a broadcast join, a pure function of (nleft, R = gathered right rows): count[32] |
 // gathered right keys [R] | gathered right payloads [R] | local join scratch.  Every rank's gathered
 // columns sit at the same offsets, so every rank knows where its slice goes inside every peer (element
-// offset: the right rows of the ranks before it), and every rank can check every rank's fit.
+// offset: the right rows of the ranks before it), and every rank can check every rank's fit.  A full
+// outer join (`full`) puts two more arrays before the scratch: matched [(R + 31) / 32] words, one bit per
+// gathered row that this rank's left rows matched, and the inbox [world][row_words] of the words every
+// rank sends for this rank's slice, row_words = (nright + 31) / 32 + 1 for this rank's nright.  The
+// inbox's offset depends on R alone, so a sender knows where it lies in every peer.
 struct BroadcastLayout {
-  size_t count, grk, grp, scratch, need;
+  size_t count, grk, grp, matched, inbox, scratch, need;
+  int64_t row_words;
 };
-static BroadcastLayout broadcast_layout(int64_t nl, int64_t R)
+static BroadcastLayout broadcast_layout(int64_t nl, int64_t R, bool full = false, int64_t nright = 0, int world = 1)
 {
   BroadcastLayout L{};
   Arena va(reinterpret_cast<void*>(4096), ~(size_t)0 >> 1);  // offsets only
@@ -1759,12 +1770,17 @@ static BroadcastLayout broadcast_layout(int64_t nl, int64_t R)
   L.count   = off(va.take<int64_t>(32));
   L.grk     = off(va.take<int64_t>((size_t)R));
   L.grp     = off(va.take<int64_t>((size_t)R));
+  if (full) {
+    L.row_words = (nright + 31) / 32 + 1;
+    L.matched   = off(va.take<uint32_t>((size_t)(R + 31) / 32));
+    L.inbox     = off(va.take<uint32_t>((size_t)world * (size_t)L.row_words));
+  }
   L.scratch = align_up(va.used, 256);
   // the ABI's workspace query does not depend on the kind: the larger of the inner and a filter kind
-  const size_t join = R <= DJ_BROADCAST_TABLE_MAX_ROWS
-                        ? broadcast_table_bytes(R)
-                        : std::max(local_join_workspace(0, R, nl), local_join_workspace(DJ_JOIN_LEFT_SEMI, R, nl)) +
-                            8192;
+  size_t join = R <= DJ_BROADCAST_TABLE_MAX_ROWS
+                  ? broadcast_table_bytes(R, full ? DJ_JOIN_FULL_OUTER : 0)
+                  : std::max(local_join_workspace(0, R, nl), local_join_workspace(DJ_JOIN_LEFT_SEMI, R, nl)) + 8192;
+  if (full && R > DJ_BROADCAST_TABLE_MAX_ROWS) join = std::max(join, broadcast_radix_mark_bytes(nl, R) + 8192);
   L.need = L.scratch + join;
   return L;
 }
@@ -1774,15 +1790,29 @@ extern "C" size_t dj_broadcast_join_workspace_bytes(int64_t nleft, int64_t nrigh
   return broadcast_layout(std::max<int64_t>(nleft, 0), std::max<int64_t>(nright_total, 0)).need;
 }
 
+extern "C" size_t dj_broadcast_full_outer_join_workspace_bytes(int64_t nleft, int64_t nright, int64_t nright_total,
+                                                               int world)
+{
+  return broadcast_layout(std::max<int64_t>(nleft, 0), std::max<int64_t>(nright_total, 0), true,
+                          std::max<int64_t>(nright, 0), std::max(world, 1))
+    .need;
+}
+
 // The local join of a broadcast join, chosen from R alone so that every rank takes the same path: the
 // hash table while it is small enough to stay in L2, else the radix-partitioned join of that kind with
-// the gathered right table as the build side (out = left ++ right).
+// the gathered right table as the build side (out = left ++ right).  A full outer join runs as a left
+// outer join that also sets d_matched (dj_internal.h).
 static int broadcast_local_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* grk,
                                 const int64_t* grp, int64_t R, int64_t* const out[4], uint8_t* out_sides,
-                                int64_t out_capacity, int64_t* d_count, Arena& arena, cudaStream_t st)
+                                int64_t out_capacity, int64_t* d_count, Arena& arena, cudaStream_t st,
+                                uint32_t* d_matched = nullptr)
 {
   if (R <= DJ_BROADCAST_TABLE_MAX_ROWS)
-    return broadcast_hash_join(kind, lk, lp, nl, grk, grp, R, out, out_sides, out_capacity, d_count, arena, st);
+    return broadcast_hash_join(kind, lk, lp, nl, grk, grp, R, out, out_sides, out_capacity, d_count, arena, st,
+                               d_matched);
+  if (kind == DJ_JOIN_FULL_OUTER)
+    return broadcast_radix_mark_join(lk, lp, nl, grk, grp, R, out, out_sides, out_capacity, d_count, d_matched, arena,
+                                     st);
   if (nl == 0) return DJ_OK;
   return local_join(kind, lk, lp, nl, grk, grp, R, out, out_sides, out_capacity, d_count, true, arena, st);
 }
@@ -1790,13 +1820,16 @@ static int broadcast_local_join(int kind, const int64_t* lk, const int64_t* lp, 
 // Every rank all-gathers the right table into the same place of its workspace and joins its own left
 // rows against it.  Steps: one hello (sizes, workspace, kind), the fit verdict from the layout, the
 // peer mappings, the pushes of this rank's right slice into every peer (copy engines and a data flag,
-// or grouped NCCL), the local join once every slice has landed, and the overflow verdict.
+// or grouped NCCL), the local join once every slice has landed, and the overflow verdict.  A full
+// outer join adds two steps between the local join and the verdict: every rank sends every peer the
+// words of its match bits that cover the peer's slice (copy engines and a second data flag, or
+// grouped NCCL), and emits the rows of its own slice whose bit no rank set.
 static int broadcast_join(dj_comm_t* comm, int kind, const int64_t* d_left_key, const int64_t* d_left_payload,
                           int64_t nleft, const int64_t* d_right_key, const int64_t* d_right_payload, int64_t nright,
                           int64_t* const out[4], uint8_t* d_out_sides, int64_t out_capacity, int64_t* h_out_count,
                           dj_join_options* opts, void* d_workspace, size_t workspace_bytes, cudaStream_t st)
 {
-  const bool filter = kind_is_filter(kind);
+  const bool filter = kind_is_filter(kind), full = kind == DJ_JOIN_FULL_OUTER;
   const int world   = comm ? comm->size : 1;
   const int rank    = comm ? comm->rank : 0;
   const size_t row_bytes = filter ? 8 : 16;  // the key column, and the payload column unless semi / anti
@@ -1805,7 +1838,7 @@ static int broadcast_join(dj_comm_t* comm, int kind, const int64_t* d_left_key, 
 
   if (world == 1) {
     DJ_REQUIRE(nright < ((int64_t)1 << 31), "broadcast_join: the right table is limited to 2^31 rows");
-    const BroadcastLayout L = broadcast_layout(nleft, nright);
+    const BroadcastLayout L = broadcast_layout(nleft, nright, full, nright, 1);
     if (workspace_bytes < L.need) {
       if (opts) opts->workspace_needed = (int64_t)L.need;
       set_error("broadcast_join: workspace too small (%zu of %zu bytes)", workspace_bytes, L.need);
@@ -1821,9 +1854,13 @@ static int broadcast_join(dj_comm_t* comm, int kind, const int64_t* d_left_key, 
         DJ_CUDA_TRY(cudaMemcpyAsync(grp, d_right_payload, (size_t)nright * 8, cudaMemcpyDeviceToDevice, st));
     }
     Arena arena(wsb + L.scratch, workspace_bytes - L.scratch);
+    uint32_t* matched = full ? (uint32_t*)(wsb + L.matched) : nullptr;
     int rc = broadcast_local_join(kind, d_left_key, d_left_payload, nleft, grk, grp, nright, out, d_out_sides,
-                                  out_capacity, d_count, arena, st);
+                                  out_capacity, d_count, arena, st, matched);
     if (rc) return rc;
+    if (full && (rc = broadcast_emit_unmatched_right(d_right_key, d_right_payload, nright, matched, 1, 0, 0, out,
+                                                     d_out_sides, out_capacity, d_count, st)))
+      return rc;
     int64_t n = 0;
     DJ_CUDA_TRY(cudaMemcpyAsync(&n, d_count, 8, cudaMemcpyDeviceToHost, st));
     DJ_CUDA_TRY(cudaStreamSynchronize(st));
@@ -1842,9 +1879,9 @@ static int broadcast_join(dj_comm_t* comm, int kind, const int64_t* d_left_key, 
   }
   DJ_REQUIRE(R < ((int64_t)1 << 31), "broadcast_join: the gathered right table (%lld rows) is limited to 2^31 rows",
              (long long)R);
-  const BroadcastLayout L = broadcast_layout(nleft, R);
+  const BroadcastLayout L = broadcast_layout(nleft, R, full, nright, world);
   for (int r = 0; r < world; r++) {
-    const size_t need = broadcast_layout(H(r, 0), R).need;
+    const size_t need = broadcast_layout(H(r, 0), R, full, H(r, 1), world).need;
     if (need > (size_t)H(r, 2)) {
       if (opts) opts->workspace_needed = (int64_t)L.need;
       set_error("broadcast_join: workspace too small on rank %d (%zu of %lld bytes; this rank needs %zu)", r, need,
@@ -1912,14 +1949,61 @@ static int broadcast_join(dj_comm_t* comm, int kind, const int64_t* d_left_key, 
 
   // ---- local join of this rank's left rows against the gathered right table
   Arena arena(wsb + L.scratch, workspace_bytes - L.scratch);
+  uint32_t* matched = full ? (uint32_t*)(wsb + L.matched) : nullptr;
   rc = broadcast_local_join(kind, d_left_key, d_left_payload, nleft, grk, grp, R, out, d_out_sides, out_capacity,
-                            d_count, arena, st);
+                            d_count, arena, st, matched);
   if (rc) return rc;
 
+  // ---- full outer: every rank's match bits for this rank's slice, then the rows nobody matched
+  if (full) {
+    std::vector<int64_t> at(world + 1, 0);  // first gathered row of every rank
+    for (int r = 0; r < world; r++) at[r + 1] = at[r] + H(r, 1);
+    auto words_for = [&](int r) { return slice_bit_words(at[r], H(r, 1)); };
+    auto row_of    = [&](int r) { return (H(r, 1) + 31) / 32 + 1; };  // the inbox row length of rank r
+    uint32_t* inbox = (uint32_t*)(wsb + L.inbox);
+    const int64_t mine = words_for(rank);
+    if (mine > 0)  // this rank's own row
+      DJ_CUDA_TRY(cudaMemcpyAsync(inbox + (size_t)rank * L.row_words, matched + (before >> 5), (size_t)mine * 4,
+                                  cudaMemcpyDeviceToDevice, st));
+    if (use_peer) {
+      DJ_CUDA_TRY(cudaEventRecord(comm->ev_ready, st));  // `matched` is complete
+      for (int k = 1; k < world; k++) {
+        const int i     = (rank + k) % world;
+        cudaStream_t ps = comm->peer_stream[i];
+        DJ_CUDA_TRY(cudaStreamWaitEvent(ps, comm->ev_ready, 0));
+        if (words_for(i) > 0)
+          DJ_CUDA_TRY(cudaMemcpyAsync(peer_ws[i] + L.inbox + (size_t)rank * row_of(i) * 4, matched + (at[i] >> 5),
+                                      (size_t)words_for(i) * 4, cudaMemcpyDefault, ps));
+        if ((rc = raise_peer_flag(comm, ps, i, kBroadcastBitsFlagSlot, seq))) return rc;  // also with no words
+      }
+      for (int src = 0; src < world; src++) {
+        if (src == rank) continue;
+        if ((rc = stream_wait_flag(comm, st, comm->d_flags + (size_t)src * kFlagSlots + kBroadcastBitsFlagSlot, seq)))
+          return rc;
+      }
+    } else {
+      DJ_NCCL_TRY(ncclGroupStart());
+      for (int i = 0; i < world; i++) {
+        if (i == rank) continue;
+        if (words_for(i) > 0)
+          DJ_NCCL_TRY(ncclSend(matched + (at[i] >> 5), (size_t)words_for(i) * 4, ncclInt8, i, comm->nccl, st));
+        if (mine > 0)
+          DJ_NCCL_TRY(ncclRecv(inbox + (size_t)i * L.row_words, (size_t)mine * 4, ncclInt8, i, comm->nccl, st));
+      }
+      DJ_NCCL_TRY(ncclGroupEnd());
+    }
+    for (int i = 0; i < world && opts; i++)
+      if (i != rank) opts->bytes_sent += words_for(i) * 4;
+    rc = broadcast_emit_unmatched_right(d_right_key, d_right_payload, nright, inbox, world, L.row_words,
+                                        (int)(before & 31), out, d_out_sides, out_capacity, d_count, st);
+    if (rc) return rc;
+  }
+
   // ---- overflow verdict.  Besides agreeing on DJ_ERR_OVERFLOW, it keeps a fast rank from pushing the
-  //      NEXT call's right slice into a peer that is still probing this call's gathered columns: a
-  //      rank's verdict is posted behind its join on its stream, and no rank returns before it has
-  //      received every peer's verdict.
+  //      NEXT call's right slice into a peer that is still probing this call's gathered columns, and
+  //      (full outer) the next call's match bits into a peer that is still emitting from this call's
+  //      inbox: a rank's verdict is posted behind its join and emit on its stream, and no rank returns
+  //      before it has received every peer's verdict.
   int64_t* h_res = comm->h_pinned + (128 << 10);
   if (use_peer && (rc = post_and_await_verdicts(comm, st, d_count, out_capacity, seq, h_res))) return rc;
   DJ_CUDA_TRY(cudaMemcpyAsync(h_res, d_count, 8, cudaMemcpyDeviceToHost, st));
@@ -1951,5 +2035,25 @@ extern "C" int dj_broadcast_join_i64(dj_comm_t* comm, int kind, const int64_t* d
   int64_t* const out[4] = {d_out_lk, d_out_lp, d_out_rk, d_out_rp};
   return broadcast_join(comm, kind, d_left_key, d_left_payload, nleft, d_right_key, d_right_payload, nright, out,
                         d_out_sides, out_capacity, h_out_count, opts, d_workspace, workspace_bytes,
+                        (cudaStream_t)stream);
+}
+
+extern "C" int dj_broadcast_full_outer_join_i64(dj_comm_t* comm, const int64_t* d_left_key,
+                                                const int64_t* d_left_payload, int64_t nleft,
+                                                const int64_t* d_right_key, const int64_t* d_right_payload,
+                                                int64_t nright, int64_t* d_out_lk, int64_t* d_out_lp,
+                                                int64_t* d_out_rk, int64_t* d_out_rp, uint8_t* d_out_sides,
+                                                int64_t out_capacity, int64_t* h_out_count, dj_join_options* opts,
+                                                void* d_workspace, size_t workspace_bytes, void* stream)
+{
+  DJ_REQUIRE(nleft >= 0 && nright >= 0 && out_capacity >= 0 && h_out_count && d_workspace,
+             "broadcast_full_outer_join: bad argument");
+  DJ_REQUIRE((nleft == 0 || (d_left_key && d_left_payload)) && (nright == 0 || (d_right_key && d_right_payload)),
+             "broadcast_full_outer_join: bad input columns");
+  DJ_REQUIRE(out_capacity == 0 || (d_out_lk && d_out_lp && d_out_rk && d_out_rp && d_out_sides),
+             "broadcast_full_outer_join: bad output columns");
+  int64_t* const out[4] = {d_out_lk, d_out_lp, d_out_rk, d_out_rp};
+  return broadcast_join(comm, DJ_JOIN_FULL_OUTER, d_left_key, d_left_payload, nleft, d_right_key, d_right_payload,
+                        nright, out, d_out_sides, out_capacity, h_out_count, opts, d_workspace, workspace_bytes,
                         (cudaStream_t)stream);
 }

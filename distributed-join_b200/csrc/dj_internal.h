@@ -279,11 +279,27 @@ int single_rank_result(int64_t n, int64_t out_capacity, int64_t* h_out_count);
 // (rk, rp)[nr], nr <= DJ_BROADCAST_TABLE_MAX_ROWS, probed by the left columns (lk, lp)[nl] in place.
 // kind 0 / DJ_JOIN_LEFT_SEMI / DJ_JOIN_LEFT_ANTI / DJ_JOIN_LEFT_OUTER; out and out_sides as for the
 // repartitioned join of that kind (rp, out[2..3] and out_sides unused by semi / anti); appends at the
-// running *d_out_count.  Takes broadcast_table_bytes(nr) from `arena`.
-size_t broadcast_table_bytes(int64_t nr);
+// running *d_out_count.  Takes broadcast_table_bytes(nr, kind) from `arena`.  DJ_JOIN_FULL_OUTER
+// writes the left outer join and sets d_matched, (nr + 31) / 32 words: bit g for every right row g that
+// some left row matched.
+size_t broadcast_table_bytes(int64_t nr, int kind = 0);
 int broadcast_hash_join(int kind, const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* rk,
                         const int64_t* rp, int64_t nr, int64_t* const out[4], uint8_t* out_sides,
-                        int64_t out_capacity, int64_t* d_out_count, Arena& arena, cudaStream_t stream);
+                        int64_t out_capacity, int64_t* d_out_count, Arena& arena, cudaStream_t stream,
+                        uint32_t* d_matched = nullptr);
+// The same left outer join and d_matched on the radix path (any nr): the kJoinFullOuterMark join of the
+// left table with (grk, gathered row index), the marks translated to rows, the pairs' right payloads
+// taken from grp.  Takes at most broadcast_radix_mark_bytes(nl, nr) from `arena`.
+size_t broadcast_radix_mark_bytes(int64_t nl, int64_t nr);
+int broadcast_radix_mark_join(const int64_t* lk, const int64_t* lp, int64_t nl, const int64_t* grk,
+                              const int64_t* grp, int64_t nr, int64_t* const out[4], uint8_t* out_sides,
+                              int64_t out_capacity, int64_t* d_out_count, uint32_t* d_matched, Arena& arena,
+                              cudaStream_t stream);
+// Appends the rows of (rk, rp)[n] whose bit is clear in all `rows` rows of `inbox` (row_words words
+// apart; row i's bit is bit0 + i) as (0, 0, key, payload) with sides DJ_SIDE_RIGHT, at the running count.
+int broadcast_emit_unmatched_right(const int64_t* rk, const int64_t* rp, int64_t n, const uint32_t* inbox, int rows,
+                                   int64_t row_words, int bit0, int64_t* const out[4], uint8_t* out_sides,
+                                   int64_t out_capacity, int64_t* d_out_count, cudaStream_t stream);
 
 // One kernel of each translation unit's module (partition.cu, join.cu, generate.cu, broadcast.cu):
 // comm.cu loads every function of these modules before ranks can wait on each other.

@@ -86,6 +86,7 @@ ABI_SYMBOLS = [
     "dj_distributed_left_filter_join_host_workspace_bytes", "dj_distributed_left_filter_join_i64_host",
     "dj_distributed_outer_join_host_workspace_bytes", "dj_distributed_outer_join_i64_host",
     "dj_broadcast_join_workspace_bytes", "dj_broadcast_join_i64",
+    "dj_broadcast_full_outer_join_workspace_bytes", "dj_broadcast_full_outer_join_i64",
 ]
 
 _lib = None
@@ -154,6 +155,10 @@ def lib() -> C.CDLL:
     L.dj_broadcast_join_workspace_bytes.restype = sz
     L.dj_broadcast_join_workspace_bytes.argtypes = [i64, i64]
     L.dj_broadcast_join_i64.argtypes = L.dj_distributed_outer_join_i64.argtypes
+    L.dj_broadcast_full_outer_join_workspace_bytes.restype = sz
+    L.dj_broadcast_full_outer_join_workspace_bytes.argtypes = [i64, i64, i64, C.c_int]
+    L.dj_broadcast_full_outer_join_i64.argtypes = [vp, vp, vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, i64,
+                                                   C.POINTER(i64), C.POINTER(JoinOptions), vp, sz, vp]
     L.dj_comm_create_local_group.argtypes = [C.c_int, C.POINTER(vp)]
     L.dj_testing_radix_repairs.argtypes = [C.POINTER(i64)]
     _lib = L
@@ -542,6 +547,34 @@ def distributed_broadcast_join(comm, kind, lk, lp, rk, rp=None, capacity=None, w
         total_right = sum(comm.allgather_i64([nr])) if world > 1 else nr
         ws_bytes = lib().dj_broadcast_join_workspace_bytes(nl, total_right)
     return _collective_join(comm, call, ncols, capacity, ws, ws_bytes, outs, lk.device)
+
+
+def distributed_broadcast_full_outer_join(comm, lk, lp, rk, rp, capacity=None, ws=None, outs=None):
+    """Broadcast FULL OUTER JOIN through dj_broadcast_full_outer_join_i64: every rank all-gathers the right
+    table, returns the left outer join of its OWN left rows (lk, lp) with the union of every rank's right
+    rows, and the rows of its own right slice (rk, rp) that no rank's left rows matched (sides SIDE_RIGHT,
+    left columns 0).  Returns a JoinResult with 5 columns (the sides column last), trimmed.  The workspace
+    is sized from this rank's right rows, the gathered right rows and the rank count; `outs`: four int64
+    columns and one uint8 column, caller-owned, for the first attempt.  Both retry loops are collective."""
+    lk, lp, rk, rp = map(_i64dev, (lk, lp, rk, rp))
+    nl, nr = lk.numel(), rk.numel()
+    world = comm.size if comm else 1
+    if capacity is None:
+        capacity = max(nl + nr, 1)
+
+    def call(outs, capacity, ws):
+        cnt = C.c_int64(0)
+        opts = JoinOptions(1, 0)
+        rc = lib().dj_broadcast_full_outer_join_i64(comm.handle if comm else None, _ptr(lk), _ptr(lp), nl, _ptr(rk),
+                                                    _ptr(rp), nr, *[_ptr(o) for o in outs], capacity, C.byref(cnt),
+                                                    C.byref(opts), _ptr(ws), ws.numel(), _stream())
+        return rc, cnt.value, opts
+
+    ws_bytes = None
+    if ws is None:
+        total_right = sum(comm.allgather_i64([nr])) if world > 1 else nr
+        ws_bytes = lib().dj_broadcast_full_outer_join_workspace_bytes(nl, nr, total_right, world)
+    return _collective_join(comm, call, 5, capacity, ws, ws_bytes, outs, lk.device)
 
 
 def _host_join(comm, name, call, ws, ws_bytes):

@@ -348,7 +348,9 @@ int dj_distributed_outer_join_i64_host(dj_comm_t* comm, int kind,
  *   - DJ_JOIN_LEFT_OUTER: the four columns plus d_out_sides, as dj_distributed_outer_join_i64 writes
  *     them (3 for a pair, 1 with zeroed right columns for a left row without a match).
  *   - DJ_JOIN_FULL_OUTER and any other kind: DJ_ERR_ARG on every rank before anything is exchanged
- *     (a right row is unmatched only once every rank's match bits are known).
+ *     (a right row is unmatched only once every rank's match bits are known; the broadcast full outer
+ *     join is its own entry, dj_broadcast_full_outer_join_i64 below, whose workspace also holds the
+ *     peers' match bits).
  * Placement: rank r returns the join of its own left rows with the gathered right table, in
  * unspecified row order; the union over the ranks is the global join.  This differs from the
  * repartitioned joins, which place rows by murmur3 owner.  comm NULL or size 1: a local join of the
@@ -380,6 +382,42 @@ int dj_broadcast_join_i64(dj_comm_t* comm, int kind,
                           int64_t* d_out_lk, int64_t* d_out_lp, int64_t* d_out_rk, int64_t* d_out_rp,
                           uint8_t* d_out_sides, int64_t out_capacity, int64_t* h_out_count,
                           dj_join_options* opts, void* d_workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------
+ * dj_broadcast_full_outer_join_i64 -- the broadcast join's FULL OUTER JOIN.  Every rank all-gathers the
+ * right table as dj_broadcast_join_i64 does, joins its own left rows against it, and records which
+ * gathered right rows they matched (one bit per gathered row).  Every rank then sends every peer the
+ * bits that cover the peer's right slice, and each rank emits the rows of its own slice that no rank's
+ * left rows matched.  Rank r returns:
+ *   - the left outer join of its own left rows with the gathered right table, exactly as
+ *     dj_broadcast_join_i64(DJ_JOIN_LEFT_OUTER) returns it (sides 3 for a pair, 1 for a left row
+ *     without a match);
+ *   - every row of its own right slice whose key no left row of ANY rank holds, as (0, 0, key, payload)
+ *     with sides DJ_SIDE_RIGHT (2).
+ * Rows come in unspecified order.  The union over the ranks is the global full outer join, and each
+ * unmatched right row appears once, on the rank that passed it in.  comm NULL or size 1: the full
+ * outer join of the two tables.  All five output columns are required (when out_capacity > 0).
+ * Collective behaviour, the local-join paths, the 256-byte workspace alignment at size > 1 and the
+ * 2^31-row limit on the gathered table are dj_broadcast_join_i64's; the kind word of the call's
+ * hello differs from every other entry's, so a rank inside this entry whose peer is inside
+ * dj_broadcast_join_i64 or a repartitioned join gets DJ_ERR_ARG on every rank.  DJ_ERR_WORKSPACE sets
+ * opts->workspace_needed to this rank's need; DJ_ERR_OVERFLOW comes with an exact *h_out_count, and
+ * nothing is written past out_capacity in any column.  opts->over_decom_factor is ignored.
+ * opts->bytes_sent is this rank's right slice and match bits sent to its peers:
+ *   (size - 1) * nright * 16 + 4 * sum over peers p of words(before_p, nright_p),
+ * where before_p is the right rows of the ranks before p, and words(b, n) = 0 for n = 0, otherwise
+ * ((b + n + 31) >> 5) - (b >> 5): the 32-bit words of the gathered bitmap that cover p's slice.
+ * Workspace: nleft, this rank's nright, the gathered row count and the rank count (the inbox of the
+ * peers' match bits holds size * ((nright + 31) / 32 + 1) words); at least
+ * dj_broadcast_join_workspace_bytes(nleft, nright_total).
+ */
+size_t dj_broadcast_full_outer_join_workspace_bytes(int64_t nleft, int64_t nright, int64_t nright_total, int world);
+int dj_broadcast_full_outer_join_i64(dj_comm_t* comm,
+                                     const int64_t* d_left_key, const int64_t* d_left_payload, int64_t nleft,
+                                     const int64_t* d_right_key, const int64_t* d_right_payload, int64_t nright,
+                                     int64_t* d_out_lk, int64_t* d_out_lp, int64_t* d_out_rk, int64_t* d_out_rp,
+                                     uint8_t* d_out_sides, int64_t out_capacity, int64_t* h_out_count,
+                                     dj_join_options* opts, void* d_workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * Testing: an in-process rank group.  Creates `size` communicators (ranks 0..size-1) on the
